@@ -3,6 +3,7 @@
 configs[1] (80 pyramids x 20 levels); the reference file's own 14 x 14 x 10 size is reported in `other_configs`.
 
   python bench.py --gpus 1 --steps K --warmup W            our CUDA path (one JSON line)
+  ... --dump-outputs DIR                                    + body states after the K-th timed step (DIR/pose.npy, DIR/vel.npy)
   python bench.py --impl reference --steps K --warmup W     CPU arm (oracle port, all host threads)
   torchrun --nproc-per-node N bench.py --gpus N ...         weak scaling: N x the scene, sharded by island
 
@@ -10,7 +11,7 @@ A "step" is one PhysicsPipeline::step of the whole scene.  `value` times steps w
 resident in HBM (CUDA events on the launching stream, max over ranks); `e2e` times the same steps
 through rb_world_step_host with HOST state buffers (H2D of every body state + D2H of the result in
 the timed region).  The reference arm is the CPU oracle (`oracle/`, a scalar restatement -- the Rust
-reference cannot be built in this image, see DESIGN.md), built -O3 -march=native on the host it runs on and run
+reference is not built by this project, see DESIGN.md), built -O3 -march=native on the host it runs on and run
 with the thread count that is fastest for the scene (swept; the sweep is printed).
 """
 import argparse
@@ -38,7 +39,7 @@ def scene_for(name, replicas=1):
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region (a throttled run is visible in the result)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -123,17 +124,6 @@ def best_cpu_world(scene, budget_s=8.0):
     return w, best[0], sweep
 
 
-def csrc_sha1():
-    """Hash of the kernel sources: ties profiles/traffic.json to the build it was measured on."""
-    import hashlib
-    h = hashlib.sha1()
-    d = os.path.join(ROOT, "rapier_b200", "csrc")
-    for f in sorted(os.listdir(d)):
-        if f.endswith((".cu", ".cuh")):
-            h.update(open(os.path.join(d, f), "rb").read())
-    return h.hexdigest()
-
-
 def algorithmic_bytes(m, b, j):
     """SURVEY.md 8(d) / BASELINE.md 4: streaming model, f32, twist friction, p = 4, S = 4."""
     return 12076 * m + 1608 * b + 6576 * j
@@ -163,7 +153,7 @@ def run_reference(args):
                          "sample": f"{args.steps} consecutive steps of the full scene after {max(args.warmup, 3)} warm-up steps; -O3 -march=native build of the oracle sources, best of the thread sweep",
                          "thread_sweep_steps_per_s": sweep, "host_cores": host_threads()},
         "e2e": {"value": value, "unit": "steps/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
-        "note": "CPU restatement (oracle/), not the reference binary: no Rust toolchain in this image. value = steps/s of ONE replica of the workload on all host threads; under weak scaling (N replicas) a CPU's replica-steps/s stay the same, so it is the comparable whole-job figure for every N",
+        "note": "CPU restatement (oracle/), not the reference binary. value = steps/s of ONE replica of the workload on all host threads; under weak scaling (N replicas) a CPU's replica-steps/s stay the same, so it is the comparable whole-job figure for every N",
     }
     print(json.dumps(line), flush=True)
 
@@ -184,6 +174,8 @@ def main():
                     help="b3d_many_pyramids_80x20 = BASELINE.json configs[1] (headline); b3d_many_pyramids = the reference file's 14x14x10")
     ap.add_argument("--l2", default="flush", choices=["flush", "keep"])
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the body states after the last timed step as DIR/pose.npy (n x 7) and DIR/vel.npy (n x 6), float32")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -260,6 +252,11 @@ def main():
         # per-launch-group device times for the roofline (events inside the library, same stream)
         if exchange is not None:
             shard.finish()   # no gather may be in flight while steps run without exchange() in between
+        if args.dump_outputs and rank == 0:   # what a caller of the timed path receives after its last step
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            pose, vel = pipe.body_states()
+            np.save(os.path.join(args.dump_outputs, "pose.npy"), pose)
+            np.save(os.path.join(args.dump_outputs, "vel.npy"), vel)
         pipe.enable_profiling(True)
         prof = {"collision_detection_ms": 0.0, "solver_ms": 0.0}
         nprof = min(args.steps, 100)
@@ -324,17 +321,10 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))   # fallback: H100 SXM data-sheet HBM3 bandwidth, not a measurement
     achieved = a_bytes / (solve_ms * 1e-3) / 1e9 if solve_ms > 0 else None
-    traffic = None
     st = pipe.debug_read("state", np.int32)
     kernel_name = "k_solve_coop_big" if int(st[19]) > 0 else "k_solve_coop"   # streamed items => the big launch shape ran
-    try:   # ncu dram bytes of THIS build (profiles/traffic.json carries the hash of the kernel sources it was captured from), else null
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        if tj.get("csrc_sha1") == csrc_sha1():
-            traffic = tj.get(f"{kernel_name}_dram_bytes_per_launch:{args.scene}")
-    except Exception:
-        pass
 
     # the reference file's own size of the same scene (14 x 14 pyramids of base 10), reported beside the headline
     other = None
@@ -381,9 +371,9 @@ def main():
             "gpu_launches": int(k1 - k0),
             "clocks": clocks,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": (achieved / peak) if achieved else None, "traffic": traffic,
+                         "frac": (achieved / peak) if achieved else None,
                          "kernel": kernel_name, "kernel_ms": solve_ms, "algorithmic_bytes_per_launch": a_bytes,
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet, 3350 GB/s (not measured)",
                          "note": "algorithmic bytes = streaming model of SURVEY 8(d); the working set is L2/shared-memory resident, see DESIGN.md"},
             "cpu_baseline": cpu,
             "stage_ms": {"collide": prof["collision_detection_ms"], "solve": prof["solver_ms"]},

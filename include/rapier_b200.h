@@ -1,4 +1,4 @@
-/* rapier_b200.h -- C ABI of librapier_b200.so, the B200-native replacement for the per-step
+/* rapier_b200.h -- C ABI of librapier_b200.so, the H100-native (sm_90a) replacement for the per-step
  * hot path of dimforge/rapier 0.35.2 (3-D, f32).
  *
  * The reference has no FFI layer for this path: the seam is the Rust method

@@ -93,6 +93,6 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  rapier_b200 has no CPU fallback.")
+                "(nvcc, sm_90a).  rapier_b200 has no CPU fallback.")
         _lib = declare(C.CDLL(LIB_PATH))
     return _lib

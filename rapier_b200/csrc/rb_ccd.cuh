@@ -145,8 +145,8 @@ RB_HD bool ccd_is_moving_fast(const Params& P, vec3 lcom, const pose& op, const 
 
 // sweep_fast_body + apply_clamps for one fast, non-bullet body: the earliest impact of any of its colliders against
 // the fixed colliders, and the pose at that fraction of the body's own sweep.  One thread; fast bodies are rare.
-// (Always inlined: as an out-of-line call inside k_collide -- ABI call, 900 B more stack -- it cost 7 us per step on the headline
-//  workload without ever being executed; inlined it costs 0.4 us: profiles/bench_r02m_ccd_placement.txt.)
+// (Always inlined: as an out-of-line call inside k_collide -- ABI call, 900 B more stack -- it costs time on every step of the
+//  headline workload even when it is never executed.)
 RB_HD pose ccd_clamp_body(const World& w, int b, pose op, pose np, bool bullet = false) {
     const State* st = w.st;
     const vec3 lcom = xyz(w.b_lcom_im[b]);

@@ -168,7 +168,7 @@ RB_PHASE unsigned long long* grid_radix_sort(const Ctx& ctx, unsigned long long*
     RB_SHARED int s_tot[RADIX];
     const int passes = radix_passes(lo, hi);
     // CTAs that take part: at least 1024 keys each (a handful of keys spread over every CTA only lengthens the
-    // per-digit walk over the CTAs' histograms below: 148 dependent L2 reads per pass); the others hold empty chunks
+    // per-digit walk over the CTAs' histograms below: one dependent L2 read per CTA per pass); the others hold empty chunks
     const int nblocks = ctx.nblocks < (n + 1023) / 1024 ? ctx.nblocks : ((n + 1023) / 1024 > 0 ? (n + 1023) / 1024 : 1);
     const int chunk = (n + nblocks - 1) / nblocks > 0 ? (n + nblocks - 1) / nblocks : 1;
     const int nwarps = ctx.bsize / ctx.nlanes < RADIX_MAX_WARPS ? ctx.bsize / ctx.nlanes : RADIX_MAX_WARPS;
@@ -568,7 +568,7 @@ RB_HD void reduce_manifold(const RawManifold& m, int* sel, int& nsel, float pred
 }
 
 // Polyhedron manifolds (SHAPES = 1 only).  A separating-axis search over two polyhedra is hundreds of candidate axes: one
-// thread per pair takes ~0.7 ms of dependent local-memory traffic however few pairs there are.  So the pairs that will get
+// thread per pair is a long chain of dependent local-memory traffic however few pairs there are.  So the pairs that will get
 // a full manifold this step (same tests as the per-pair loop below: an awake owned body, not recycled) are listed first,
 // then each is handed to a whole WARP (consecutive list entries to different CTAs), whose lanes share the candidate axes
 // (rb_poly.cuh) with the polyhedra staged in shared memory; the raw manifold goes to a scratch table the per-pair pass reads.
@@ -927,8 +927,8 @@ RB_PHASE void section_coloring(const Ctx& ctx, const World& w) {
 
 // ------------------------------------------------------------------------------------------------
 // Grid-wide exclusive scan of ints: per-thread chunks, a shared-memory scan of the partial sums inside every CTA, then
-// every CTA adds up the totals of the CTAs before it (no serial pass of one CTA over all the partials: that cost ~45 us
-// per scan).  `tmp` needs gsize + 1 entries.  Returns the total in tmp[gsize].
+// every CTA adds up the totals of the CTAs before it (no serial pass of one CTA over all the partials: that
+// serialises the scan).  `tmp` needs gsize + 1 entries.  Returns the total in tmp[gsize].
 // ------------------------------------------------------------------------------------------------
 template <class Ctx>
 RB_PHASE void grid_exclusive_scan(const Ctx& ctx, const int* in, int* out, int n, int* tmp) {
@@ -1136,7 +1136,7 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
     ctx.grid_sync();
     RB_CSTAMP(8);
     // S5 colour stage order: big colours ascending, then small colours ascending, then overflow.  One CTA, a thread per
-    // colour ranking itself against a shared copy of the counts (a single thread walking global memory cost ~150 us).
+    // colour ranking itself against a shared copy of the counts (a single thread walking global memory is far slower).
     if (ctx.bid == 0) {
         RB_SHARED int s_cnt[NUM_COLORS];
         for (int c = ctx.btid; c < NUM_COLORS; c += ctx.bsize) s_cnt[c] = w.color_count[c];
@@ -1258,7 +1258,7 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
     // S10a item 0 (the grid-wide islands: up to every constraint of the world) is sorted by colour stage by the WHOLE grid:
     // per-CTA histograms of contiguous chunks, totals and per-CTA bases through global atomics, scatter.  The order inside
     // a colour is arbitrary here as in S10 (constraints of one colour share no body); the overflow colour is put in index
-    // order afterwards.  One CTA took 0.3 - 0.6 ms for the 30 000 - 70 000 constraints of keva / pyramid3.
+    // order afterwards.  One CTA alone is too slow for the 30 000 - 70 000 constraints of keva / pyramid3.
     for (int pass = 0; pass < 2; ++pass) {   // 0: contacts, 1: joints
         RB_SHARED int hist0[NUM_COLORS + 1];
         RB_SHARED int offs0[NUM_COLORS + 1];

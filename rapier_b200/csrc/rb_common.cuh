@@ -2,7 +2,7 @@
 //
 // All device work is written as "phase functions": `template <class Ctx> RB_HD void phase(Ctx&, ...)`
 // whose loops are strided by the context (grid-wide, CTA-wide or warp-wide) and whose phase
-// boundaries are ctx.grid_sync() / ctx.block_sync().  The product build (nvcc, sm_100a) instantiates
+// boundaries are ctx.grid_sync() / ctx.block_sync().  The product build (nvcc, sm_90a) instantiates
 // them with the CUDA contexts below inside __global__ kernels.  tests/emul/ compiles the very same
 // phase functions with g++ and a one-thread context (RB_EMULATE) so the kernel LOGIC can be checked
 // against the oracle on a machine without a GPU; that build is test infrastructure only and is never

@@ -1,6 +1,6 @@
-// Microbenchmark (not a test): latency of a grid-wide barrier on 148 x 256 threads --
+// Microbenchmark (not a test): latency of a grid-wide barrier on one 256-thread CTA per SM (132 on an H100 SXM) --
 // cooperative_groups grid.sync() against a ticket barrier on one 64-bit counter (atomicAdd + acquire spin).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o grid_barrier grid_barrier.cu && ./grid_barrier
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o grid_barrier grid_barrier.cu && ./grid_barrier
 #include <cooperative_groups.h>
 #include <cstdio>
 namespace cg = cooperative_groups;

@@ -1,7 +1,7 @@
 // Microbenchmark behind the staging-pipeline design (DESIGN.md "streamed items"): cost of staging one
 // chunk of constraint rows (ROWS rows x cnt slots x 16 B) from an L2-resident pool into shared memory
 // with 1-D bulk (TMA) copies, as a function of who issues them and of the source alignment.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_rows tma_rows.cu && ./tma_rows
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_rows tma_rows.cu && ./tma_rows
 #include <cstdio>
 #include <cuda_runtime.h>
 constexpr int ROWS = 36;
@@ -49,17 +49,17 @@ int main() {
     const size_t gstride = 524288;   // float4 per pool row, like cons_cap of the 80x20 scene
     float4* pool; long long* out; float* sink;
     cudaMalloc(&pool, ROWS * gstride * 16); cudaMemset(pool, 0, ROWS * gstride * 16);
-    cudaMalloc(&out, 148 * 8); cudaMalloc(&sink, 4);
+    cudaMalloc(&out, 132 * 8); cudaMalloc(&sink, 4);
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     const char* names[] = {"1 thread x 36 row copies", "36 threads x 1 row copy", "1 contiguous copy", "LDG+STS by 384 threads"};
-    for (int blocks : {1, 80, 148})
+    for (int blocks : {1, 80, 132})   // 132 = one CTA per SM of an H100 SXM
         for (int cnt : {32, 96})
             for (int off : {0, 3})
                 for (int mode = 0; mode < 4; ++mode) {
                     if (mode == 2 && off) continue;
                     k<<<blocks, 384, ROWS * cnt * 16>>>(pool, gstride, cnt, off, mode, 8, out, sink);   // warm L2
                     k<<<blocks, 384, ROWS * cnt * 16>>>(pool, gstride, cnt, off, mode, 64, out, sink);
-                    long long h[148]; cudaMemcpy(h, out, blocks * 8, cudaMemcpyDeviceToHost);
+                    long long h[132]; cudaMemcpy(h, out, blocks * 8, cudaMemcpyDeviceToHost);
                     long long mx = 0; for (int i = 0; i < blocks; ++i) mx = h[i] > mx ? h[i] : mx;
                     printf("blocks=%3d cnt=%3d (%5d B/chunk) src_off=%d float4  %-26s : %6lld cycles/chunk  %s\n", blocks, cnt, ROWS * cnt * 16, off, names[mode], mx,
                            cudaGetErrorString(cudaGetLastError()));

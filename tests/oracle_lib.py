@@ -3,6 +3,7 @@ imported by tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
 import ctypes as C
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -42,8 +43,9 @@ def lib(fast=False):
         path = LIB_PATH
         if fast:
             tag = _cpu_tag()
-            path = os.path.join(ORACLE_DIR, "_build", f"liborc_fast_{tag}.so")
-            subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "fast", f"FAST_TAG={tag}"])
+            # built in a per-user temporary directory: the benchmark must not write into the source tree
+            path = os.path.join(tempfile.gettempdir(), f"rapier_b200_orc_{os.getuid()}", f"liborc_fast_{tag}.so")
+            subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "fast", f"FAST_TAG={tag}", f"FAST_OUT={path}"])
         elif not os.path.exists(LIB_PATH):
             build()
         L = C.CDLL(path)

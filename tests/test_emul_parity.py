@@ -1,6 +1,6 @@
 """Kernel LOGIC check without a GPU: the phase functions of rapier_b200/csrc compiled for the host
 (tests/emul, -DRB_EMULATE, one thread playing every CUDA thread) against the CPU oracle.  These do
-not exercise the product library; the `-m gpu` tests do that on the B200."""
+not exercise the product library; the `-m gpu` tests do that on the GPU."""
 import numpy as np
 from rapier_b200 import _abi as A
 import pytest
