@@ -17,6 +17,7 @@
 #include <algorithm>
 #include <string>
 #include <array>
+#include <type_traits>
 #include <vector>
 
 #include "rb_solver.cuh"
@@ -235,7 +236,8 @@ RB_PHASE void set_halo_phase(const Ctx& ctx, const World& w, const unsigned char
 // Collision pipeline, then every solve that is NOT shared-memory resident: work items streamed from
 // HBM (one CTA each) and the grid-wide "large" item 0.  Those touch bodies / constraints disjoint from
 // the items k_solve_coop handles next, so the order between the two kernels does not matter.
-// `do_collide` = 0 runs only the solve part (unused in the normal step).
+// `do_solve` = 0 runs only the collision pipeline (the general path, whose solves have kernels of their own);
+// bit 1 set: k_solve_large follows and solves the grid-wide item 0.
 // SHAPES = 1: the variant for worlds with capsules (rb_geom.cuh); the ball / cuboid kernel is SHAPES = 0.
 template <int SHAPES>
 __global__ void __launch_bounds__(COLLIDE_THREADS) k_collide(World w, Grav g, int do_solve) {
@@ -281,7 +283,7 @@ __global__ void __launch_bounds__(COLLIDE_THREADS) k_collide(World w, Grav g, in
             if (k >= n) break;
             const int item = w.item_order[k];
             if (item_is_coop(w, item)) continue;
-            solve_item(ex, w, bd, item, mk3(g.x, g.y, g.z));
+            solve_item<HbmRows<0, 0>>(ex, w, bd, item, mk3(g.x, g.y, g.z));
             ex.sync();
         }
     }
@@ -293,7 +295,7 @@ __global__ void __launch_bounds__(COLLIDE_THREADS) k_collide(World w, Grav g, in
     gb.w = &w;
     GridSpreadExec gex;
     gex.c = &ctx;
-    solve_item_lanes<4>(gex, w, gb, mk3(g.x, g.y, g.z));
+    solve_item<PoolRows<4>>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
 }
 // The grid-wide item 0: islands too large for one CTA (pyramid3, keva3, joint grids).  Cooperative, one CTA per SM;
 // bodies in the global solver-body tables, constant rows in the L2-resident large pool, one grid barrier per colour
@@ -305,12 +307,12 @@ __global__ void __launch_bounds__(COLLIDE_THREADS, 1) k_solve_large(World w, Gra
     gb.w = &w;
     GridSpreadExec gex;
     gex.c = &ctx;
-    solve_item_lanes<4>(gex, w, gb, mk3(g.x, g.y, g.z));
+    solve_item<PoolRows<4>>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
 }
 // The general solve path, compiled per (friction model FM, joint model JM):
 //   FM = 1  FrictionModel::Coulomb (integration_parameters.rs:26-29): one coupled tangent part per contact point
 //   JM = 1  some joint has limits or motors (joint_velocity_constraint.rs:145-357): generic joint rows
-// Every work item takes the streaming solve (solve_item<FM, JM>: bodies in shared memory, rows in HBM/L2), the
+// Every work item takes the streaming solve (solve_item<HbmRows<FM, JM>>: bodies in shared memory, rows in HBM/L2), the
 // grid-wide item 0 the same code with grid barriers.  The twist / locked-axes kernels carry none of this code.
 template <int FM, int JM>
 __global__ void __launch_bounds__(COLLIDE_THREADS) k_solve_items_x(World w, Grav g) {
@@ -328,7 +330,7 @@ __global__ void __launch_bounds__(COLLIDE_THREADS) k_solve_items_x(World w, Grav
         const int k = s_next;
         __syncthreads();
         if (k >= n) break;
-        solve_item<FM, JM>(ex, w, bd, w.item_order[k], mk3(g.x, g.y, g.z));
+        solve_item<HbmRows<FM, JM>>(ex, w, bd, w.item_order[k], mk3(g.x, g.y, g.z));
         ex.sync();
     }
 }
@@ -340,14 +342,14 @@ __global__ void __launch_bounds__(COLLIDE_THREADS, 1) k_solve_large_x(World w, G
     gb.w = &w;
     GridExec gex;
     gex.c = &ctx;
-    solve_item<FM, JM>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
+    solve_item<HbmRows<FM, JM>>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
 }
 // Shared-memory items: one CTA per item, bodies (and, when they fit, constraints) staged in shared memory,
 // four lanes per constraint (rb_solver.cuh "lane-cooperative path").
 // Either launch shape takes every shared-memory item (the small one streams what does not fit), so the
 // host's choice between them -- a hint read without synchronising -- only affects speed.
 template <int L>
-__device__ __forceinline__ void solve_coop_items(const World& w, const Grav& g, int smem_floats, bool big) {
+__device__ __forceinline__ void solve_coop_items(const World& w, const Grav& g, int smem_floats) {
     extern __shared__ __align__(16) float smem[];
     __shared__ __align__(8) unsigned long long s_mbar[2];
     BlockCtx ctx;
@@ -364,7 +366,6 @@ __device__ __forceinline__ void solve_coop_items(const World& w, const Grav& g, 
     __shared__ int s_next;
     const int n = w.st->norder;
     int* cursor = &w.st->cursor_coop;
-    (void)big;
     for (;;) {   // dynamic queue over the cost-ordered items
         if (ctx.btid == 0) s_next = atomicAdd(cursor, 1);
         __syncthreads();
@@ -378,9 +379,8 @@ __device__ __forceinline__ void solve_coop_items(const World& w, const Grav& g, 
     }
 }
 // The two launch shapes (COOP_SMALL_* / COOP_BIG_*): same code, different register budgets.
-__global__ void __launch_bounds__(COOP_SMALL_THREADS, 2) k_solve_coop(World w, Grav g) { solve_coop_items<4>(w, g, COOP_SMALL_SMEM_BYTES / 4, false); }
-template <int THREADS, int L>
-__global__ void __launch_bounds__(THREADS, 1) k_solve_coop_big(World w, Grav g) { solve_coop_items<L>(w, g, COOP_BIG_SMEM_BYTES / 4, true); }
+__global__ void __launch_bounds__(COOP_SMALL_THREADS, 2) k_solve_coop(World w, Grav g) { solve_coop_items<4>(w, g, COOP_SMALL_SMEM_BYTES / 4); }
+__global__ void __launch_bounds__(COOP_BIG_THREADS, 1) k_solve_coop_big(World w, Grav g) { solve_coop_items<1>(w, g, COOP_BIG_SMEM_BYTES / 4); }
 __global__ void k_kat(World w, int which, const float* in, float* out) { kat_phase(w, which, in, out); }
 // Contact force events of the step just solved (launched only for worlds in which a collider asks for them).
 __global__ void k_force_events(World w) {
@@ -442,9 +442,7 @@ struct RbWorld {
     int device = 0;
     int num_sms = 1;
     int collide_blocks = 1, coop_blocks = 1;
-    int collide_threads = COLLIDE_THREADS;
     int coop_blocks_big = 1;
-    int big_threads = COOP_BIG_THREADS, sweep_threads = 0;
     float* state_buf[2] = {nullptr, nullptr};   // double-buffered packed state (rb_world_state_buffers), else unused
     int state_next = 0;
     bool ext_shapes = false;     // some collider is a capsule or a convex polyhedron: the SHAPES = 1 collision kernel
@@ -495,6 +493,22 @@ static void free_all(RbWorld* W) {
 }
 
 static int next_pow2_host(int n) { int p = 1; while (p < n) p <<= 1; return p; }
+
+// The general solve path: every item, the grid-wide item 0 included, through solve_item<HbmRows<FM, JM>>.
+static bool general_path(const World& w) { return w.prm.friction_model == 1 || w.generic_joints != 0 || w.any_extra != 0; }
+// Calls f(FM, JM) with the compile-time variant of the general path as std::integral_constant values:
+// FM = 1 FrictionModel::Coulomb, JM = 1 generic joints.
+template <class F>
+static auto with_variant(bool fm, bool jm, F&& f) {
+    using I0 = std::integral_constant<int, 0>;
+    using I1 = std::integral_constant<int, 1>;
+    if (fm && jm) return f(I1(), I1());
+    if (fm) return f(I1(), I0());
+    if (jm) return f(I0(), I1());
+    return f(I0(), I0());
+}
+template <class F>
+static auto with_variant(const World& w, F&& f) { return with_variant(w.prm.friction_model == 1, w.generic_joints != 0, f); }
 
 // Derived solver coefficients (integration_parameters.rs:85-149, :305-377; init.rs:96-101).
 static void derive_params(const RbIntegrationParameters& p_in, Params& o, int extra_substeps = 0) {
@@ -1111,17 +1125,15 @@ RbWorld* rb_world_create(const RbIntegrationParameters* params, int device) {
     if (!prop.cooperativeLaunch) { set_err("device lacks cooperative launch%s", ""); delete W; return nullptr; }
     cudaStreamCreateWithFlags(&W->stream, cudaStreamNonBlocking);
     cudaFuncSetAttribute(k_solve_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, COOP_SMALL_SMEM_BYTES);
-#define RB_BIG_VARIANTS(X) X(256, 1)
-#define RB_SET_ATTR(T, LL) cudaFuncSetAttribute(k_solve_coop_big<T, LL>, cudaFuncAttributeMaxDynamicSharedMemorySize, COOP_BIG_SMEM_BYTES);
-    RB_BIG_VARIANTS(RB_SET_ATTR)
+    cudaFuncSetAttribute(k_solve_coop_big, cudaFuncAttributeMaxDynamicSharedMemorySize, COOP_BIG_SMEM_BYTES);
     if (cudaHostAlloc((void**)&W->host_hint, 4 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) { set_err("cudaHostAlloc failed%s", ""); delete W; return nullptr; }
     for (int i = 0; i < 4; ++i) W->host_hint[i] = 0;
     cudaFuncSetAttribute(k_collide<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
     cudaFuncSetAttribute(k_collide<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
-    cudaFuncSetAttribute(k_solve_items_x<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
-    cudaFuncSetAttribute(k_solve_items_x<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
-    cudaFuncSetAttribute(k_solve_items_x<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
-    cudaFuncSetAttribute(k_solve_items_x<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
+    for (int v = 0; v < 4; ++v)   // every variant: the friction model may change after the world is created
+        with_variant(v & 1, v & 2, [](auto fm, auto jm) {
+            cudaFuncSetAttribute(k_solve_items_x<decltype(fm)::value, decltype(jm)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
+        });
     int occ = 1;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_collide<1>, COLLIDE_THREADS, ITEM_SMEM_BYTES);
     if (occ < 1) { set_err("k_collide cannot be resident%s", ""); delete W; return nullptr; }
@@ -1130,13 +1142,9 @@ RbWorld* rb_world_create(const RbIntegrationParameters* params, int device) {
     if (occ < 1) occ = 1;
     W->coop_blocks = W->num_sms * occ;
     W->coop_blocks_big = W->num_sms;
-    {   // debugging overrides (never needed in production): shrink the launch geometry
-        auto envi = [](const char* n, int d) { const char* v = getenv(n); return v ? atoi(v) : d; };
-        W->collide_blocks = std::min(W->collide_blocks, envi("RB_COLLIDE_BLOCKS", W->collide_blocks));
-        W->coop_blocks = std::min(W->coop_blocks, envi("RB_COOP_BLOCKS", W->coop_blocks));
-        W->collide_threads = std::min(COLLIDE_THREADS, envi("RB_COLLIDE_THREADS", COLLIDE_THREADS));
-        W->coop_shape = envi("RB_COOP_SHAPE", -1);
-        W->sweep_threads = envi("RB_COOP_SWEEP_THREADS", 0);
+    {   // debugging override (never needed in production): force the launch shape of k_solve_coop
+        const char* v = getenv("RB_COOP_SHAPE");
+        W->coop_shape = v ? atoi(v) : -1;
     }
 #else
     {   // emulated CTA: shared-memory size of the big launch shape, or a test override that forces streaming
@@ -1384,7 +1392,6 @@ int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t
     ALLOC(w.large_pool, (size_t)COOP_ROWS * w.cons_cap); ALLOC(w.large_mut, (size_t)MR_COUNT * w.cons_cap);
     w.host_hint = W->host_hint;
     w.coop_small_floats = COOP_SMALL_SMEM_BYTES / 4;
-    w.coop_sweep_threads = W->sweep_threads;
 #ifdef RB_DEBUG
     { const char* v = getenv("RB_DEBUG_FLAGS"); w.debug_flags = v ? atoi(v) : 0; }
 #endif
@@ -1865,9 +1872,9 @@ int rb_world_step(RbWorld* W, const float gravity[3], int32_t nsteps, int32_t sy
         bool prof = W->profiling;
         if (prof) CK(cudaEventRecord(W->prof_ev[3 * s], W->stream));
         // a grid-wide island existed after the last schedule the host knows of: it gets its own launch
-        const bool coulomb = W->w.prm.friction_model == 1 || W->w.generic_joints != 0 || W->w.any_extra != 0;   // (the general solve path)
+        const bool general = general_path(W->w);
         const bool large = *(volatile int*)(W->host_hint + 2) != 0;
-        int do_solve = coulomb ? 0 : (large ? 3 : 1);
+        int do_solve = general ? 0 : (large ? 3 : 1);
         if (W->state_buf[1]) { W->w.state13 = W->state_buf[W->state_next]; W->state_next ^= 1; }
         // A new scene's islands are only known after its first schedule.  A caller that enqueues many steps in
         // one asynchronous call would otherwise run all of them in the launch shape chosen before that, so the
@@ -1878,12 +1885,10 @@ int rb_world_step(RbWorld* W, const float gravity[3], int32_t nsteps, int32_t sy
         const bool big = W->coop_shape >= 0 ? W->coop_shape == 1 : (*(volatile int*)W->host_hint != 0);
         W->w.step_index = (int)(W->steps + s + 1);
         void* a1[] = {(void*)&W->w, (void*)&g, (void*)&do_solve};
-        CK(cudaLaunchCooperativeKernel(W->ext_shapes ? (void*)k_collide<1> : (void*)k_collide<0>, dim3(W->collide_blocks), dim3(W->collide_threads), a1, ITEM_SMEM_BYTES, W->stream));
+        CK(cudaLaunchCooperativeKernel(W->ext_shapes ? (void*)k_collide<1> : (void*)k_collide<0>, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a1, ITEM_SMEM_BYTES, W->stream));
         if (prof) CK(cudaEventRecord(W->prof_ev[3 * s + 1], W->stream));
-        if (coulomb) {   // every item through the streaming solve; the grid-wide item's kernel returns at once when there is none
+        if (general) {   // every item through the streaming solve; the grid-wide item's kernel returns at once when there is none
             void* a2[] = {(void*)&W->w, (void*)&g};
-            const int fm = W->w.prm.friction_model == 1 ? 1 : 0, jm = W->w.generic_joints ? 1 : 0;
-            void* large = fm ? (jm ? (void*)k_solve_large_x<1, 1> : (void*)k_solve_large_x<1, 0>) : (jm ? (void*)k_solve_large_x<0, 1> : (void*)k_solve_large_x<0, 0>);
             // substep solve-groups: one pass of both kernels per distinct key, each with the parameters of its cadence
             const size_t npass = W->w.any_extra ? W->extra_keys.size() : 1;
             for (size_t ki = 0; ki < npass; ++ki) {
@@ -1892,11 +1897,11 @@ int rb_world_step(RbWorld* W, const float gravity[3], int32_t nsteps, int32_t sy
                     derive_params(W->params, W->w.prm, W->w.pass_key);
                     if (ki > 0) CK(cudaMemsetAsync(&W->w.st->cursor_rest, 0, sizeof(int), W->stream));
                 }
-                if (fm && jm) k_solve_items_x<1, 1><<<W->collide_blocks, W->collide_threads, ITEM_SMEM_BYTES, W->stream>>>(W->w, g);
-                else if (fm) k_solve_items_x<1, 0><<<W->collide_blocks, W->collide_threads, ITEM_SMEM_BYTES, W->stream>>>(W->w, g);
-                else if (jm) k_solve_items_x<0, 1><<<W->collide_blocks, W->collide_threads, ITEM_SMEM_BYTES, W->stream>>>(W->w, g);
-                else k_solve_items_x<0, 0><<<W->collide_blocks, W->collide_threads, ITEM_SMEM_BYTES, W->stream>>>(W->w, g);
-                CK(cudaLaunchCooperativeKernel(large, dim3(W->collide_blocks), dim3(W->collide_threads), a2, 0, W->stream));
+                CK(with_variant(W->w, [&](auto fm, auto jm) {
+                    constexpr int FM = decltype(fm)::value, JM = decltype(jm)::value;
+                    k_solve_items_x<FM, JM><<<W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, W->stream>>>(W->w, g);
+                    return cudaLaunchCooperativeKernel((void*)k_solve_large_x<FM, JM>, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a2, 0, W->stream);
+                }));
                 W->kernels += 2;
             }
             if (W->w.any_extra) { W->w.pass_key = 0; derive_params(W->params, W->w.prm); }
@@ -1907,13 +1912,11 @@ int rb_world_step(RbWorld* W, const float gravity[3], int32_t nsteps, int32_t sy
         }
         if (large) {
             void* a2[] = {(void*)&W->w, (void*)&g};
-            CK(cudaLaunchCooperativeKernel((void*)k_solve_large, dim3(W->collide_blocks), dim3(W->collide_threads), a2, 0, W->stream));
+            CK(cudaLaunchCooperativeKernel((void*)k_solve_large, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a2, 0, W->stream));
             W->kernels++;
         }
-        if (big) {
-#define RB_LAUNCH_BIG(T, LL) if (W->big_threads == T) k_solve_coop_big<T, LL><<<W->coop_blocks_big, T, COOP_BIG_SMEM_BYTES, W->stream>>>(W->w, g);
-            RB_BIG_VARIANTS(RB_LAUNCH_BIG)
-        } else k_solve_coop<<<W->coop_blocks, COOP_SMALL_THREADS, COOP_SMALL_SMEM_BYTES, W->stream>>>(W->w, g);
+        if (big) k_solve_coop_big<<<W->coop_blocks_big, COOP_BIG_THREADS, COOP_BIG_SMEM_BYTES, W->stream>>>(W->w, g);
+        else k_solve_coop<<<W->coop_blocks, COOP_SMALL_THREADS, COOP_SMALL_SMEM_BYTES, W->stream>>>(W->w, g);
         if (W->force_events) { k_force_events<<<W->collide_blocks, 256, 0, W->stream>>>(W->w); W->kernels++; }
         CK(cudaGetLastError());
         if (prof) CK(cudaEventRecord(W->prof_ev[3 * s + 2], W->stream));
@@ -1958,29 +1961,23 @@ int rb_world_step(RbWorld* W, const float gravity[3], int32_t nsteps, int32_t sy
         const size_t npass = W->w.any_extra ? W->extra_keys.size() : 1;   // substep solve-groups: one pass per distinct key
         for (size_t ki = 0; ki < npass; ++ki) {
         if (W->w.any_extra) { W->w.pass_key = W->extra_keys[ki]; derive_params(W->params, W->w.prm, W->w.pass_key); }
-        const bool grp = W->w.any_extra != 0;
+        const bool general = general_path(W->w);
         for (int k = 0; k < W->w.st->norder; ++k) {
             const int item = W->w.item_order[k];
-            const bool fm1 = W->w.prm.friction_model == 1, jm1 = W->w.generic_joints != 0;
-            if (fm1 && jm1) solve_item<1, 1>(bex, W->w, sb, item, mk3(g.x, g.y, g.z));
-            else if (fm1) solve_item<1, 0>(bex, W->w, sb, item, mk3(g.x, g.y, g.z));
-            else if (jm1) solve_item<0, 1>(bex, W->w, sb, item, mk3(g.x, g.y, g.z));
-            else if (grp) solve_item<0, 0>(bex, W->w, sb, item, mk3(g.x, g.y, g.z));
+            if (general)
+                with_variant(W->w, [&](auto fm, auto jm) { solve_item<HbmRows<decltype(fm)::value, decltype(jm)::value>>(bex, W->w, sb, item, mk3(g.x, g.y, g.z)); });
             else if (item_is_coop(W->w, item))
                 solve_item_coop<1>(bctx, W->w, W->emu_smem.data() + ITEM_MAX_BODIES * SB_STRIDE, W->emu_coop_floats, pp, item, mk3(g.x, g.y, g.z));
-            else solve_item(bex, W->w, sb, item, mk3(g.x, g.y, g.z));
+            else solve_item<HbmRows<0, 0>>(bex, W->w, sb, item, mk3(g.x, g.y, g.z));
         }
         if (W->w.st->nlarge_bodies > 0) {
             GlobalBodies gb;
             gb.w = &W->w;
             GridExec gex;
             gex.c = &gctx;
-            const bool fm1 = W->w.prm.friction_model == 1, jm1 = W->w.generic_joints != 0;
-            if (fm1 && jm1) solve_item<1, 1>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z));
-            else if (fm1) solve_item<1, 0>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z));
-            else if (jm1) solve_item<0, 1>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z));
-            else if (grp) solve_item<0, 0>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z));
-            else solve_item_lanes<1>(gex, W->w, gb, mk3(g.x, g.y, g.z));
+            if (general)
+                with_variant(W->w, [&](auto fm, auto jm) { solve_item<HbmRows<decltype(fm)::value, decltype(jm)::value>>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z)); });
+            else solve_item<PoolRows<1>>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z));
         }
         }
         if (W->w.any_extra) { W->w.pass_key = 0; derive_params(W->params, W->w.prm); }
@@ -2262,7 +2259,7 @@ int rb_world_label_components(RbWorld* W, int32_t* component_of_body) {
     Grav g0{0.f, 0.f, 0.f};
     int do_solve = 0;
     void* a1[] = {(void*)&W->w, (void*)&g0, (void*)&do_solve};
-    CK(cudaLaunchCooperativeKernel(W->ext_shapes ? (void*)k_collide<1> : (void*)k_collide<0>, dim3(W->collide_blocks), dim3(W->collide_threads), a1, ITEM_SMEM_BYTES, W->stream));
+    CK(cudaLaunchCooperativeKernel(W->ext_shapes ? (void*)k_collide<1> : (void*)k_collide<0>, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a1, ITEM_SMEM_BYTES, W->stream));
     W->kernels++;
 #else
     W->w.st->sched_dirty = 1;

@@ -1,9 +1,15 @@
 // rb_solver.cuh -- the velocity solver + integrator, fused per work item.
 //
 // One work item = a group of whole connected components ("islands").  An item is solved start to
-// finish by ONE CTA with its bodies' velocities / poses / inverse inertias staged in shared memory
-// (solve_item<BlockExec, SmemBodies>), or -- for islands too large for a CTA (item 0) -- by the
-// whole grid with bodies in HBM and grid-wide barriers (solve_item<GridExec, GlobalBodies>).
+// finish by ONE CTA with its bodies' velocities / poses / inverse inertias staged in shared memory, or
+// -- for islands too large for a CTA (item 0) -- by the whole grid with bodies in HBM and grid-wide
+// barriers.  Two step functions do it:
+//   solve_item<R>     the streaming / grid-wide solve, one skeleton over an executor (BlockExec / GridExec /
+//                     GridSpreadExec), a body store (SmemBodies / GlobalBodies) and a constraint-row policy R:
+//                     HbmRows<FM, JM> (Cons tables in HBM/L2: every item of the general path, and the items
+//                     k_collide takes) or PoolRows<L> (lane-cooperative rows in the L2 pool: the grid-wide item 0
+//                     outside the general path)
+//   solve_item_coop   the shared-memory items: bodies, impulses and (when they fit) constraint rows in shared memory
 // Either way the stage order is the reference's:
 //   S1 solver-body init   staged_island_solver/worker.rs:46-104, solver_body.rs:82-121
 //   S2 generate           contact_with_twist_friction.rs:58-424
@@ -1321,152 +1327,6 @@ RB_HD void body_writeback(const World& w, const B& bd, int b, int id) {
     s[7] = lin.x; s[8] = lin.y; s[9] = lin.z; s[10] = ang.x; s[11] = ang.y; s[12] = ang.z;
 }
 
-// Solve one work item from solver-body init to the final positions of its bodies, constraints
-// streaming from HBM/L2 (fallback for items too big for shared memory, items with joints, item 0).
-template <int FM = 0, int JM = 0, class X, class B>
-RB_PHASE void solve_item(const X& ex, const World& w, const B& bd, int item, vec3 gravity) {
-    const Params& P = w.prm;
-    State* st = w.st;
-    const int buf = st->cur;
-    const bool global_ids = item == 0;
-    const int b0 = w.item_body_start[item], b1 = w.item_body_start[item + 1];
-    const int c0 = w.item_cons_start[item];
-    const int c1 = w.item_cons_start[item + 1] < w.cons_cap ? w.item_cons_start[item + 1] : w.cons_cap;
-    const int j0 = w.item_joint_start[item], j1 = w.item_joint_start[item + 1];
-    const int* coff = w.item_color_off + (size_t)item * (NUM_COLORS + 1);
-    const int* joff = w.item_jcolor_off + (size_t)item * (NUM_COLORS + 1);
-    const int ncol = st->nused_colors, njcol = st->njused_colors;
-    const int ovf = w.color_pos[COLOR_OVERFLOW], jovf = w.jcolor_pos[COLOR_OVERFLOW];
-    const int tid = ex.tid(), nth = ex.nth();
-    // substep solve-groups: this launch solves the islands whose key is pass_key, at the cadence w.prm was derived for
-    const bool grp = w.any_extra != 0;
-    const unsigned char gk = (unsigned char)w.pass_key;
-
-    auto stage = [&](int a, int e, bool serial, int mode, bool fric) {
-        if (serial) {
-            if (tid == 0)
-                for (int q = a; q < e; ++q) { if (grp && w.cons_key[q] != gk) continue; Cons cc; cons_load<FM>(w, q, cc); cons_sweep<FM>(w, bd, q, cc, mode, fric); cons_store_dyn<FM>(w, q, cc); }
-        } else {
-            for (int q = a + tid; q < e; q += nth) { if (grp && w.cons_key[q] != gk) continue; Cons cc; cons_load<FM>(w, q, cc); cons_sweep<FM>(w, bd, q, cc, mode, fric); cons_store_dyn<FM>(w, q, cc); }
-        }
-    };
-
-    if (tid == 0) w.item_flags[item] = 0;   // bit 0: some contact of this item holds a restitution seed
-    for (int l = b0 + tid; l < b1; l += nth) {
-        int b = w.item_bodies[l];
-        if (grp && w.b_key[b] != gk) continue;
-        body_init(w, bd, b, global_ids ? b : l - b0, gravity);
-    }
-    ex.sync();
-    // S2 generate
-    for (int q = c0 + tid; q < c1; q += nth) {
-        if (grp && w.cons_key[q] != gk) continue;
-        Cons c;
-        cons_generate<FM>(w, bd, q, buf, item, c);
-        cons_store_static<FM>(w, q, c);
-        cons_store_dyn<FM>(w, q, c);
-    }
-    ex.sync();
-
-    for (int sub = 0; sub < P.num_substeps; ++sub) {
-        for (int l = b0 + tid; l < b1; l += nth) {
-            int b = w.item_bodies[l];
-            if (grp && w.b_key[b] != gk) continue;
-            body_increment(w, bd, b, global_ids ? b : l - b0);
-        }
-        ex.sync();
-        // S4 joint rows from the current poses
-        if (j1 > j0) {
-            for (int q = j0 + tid; q < j1; q += nth) { if (grp && w.j_key[q] != gk) continue; if (JM) joint_update_generic(w, bd, q, sub); else joint_update(w, bd, q); }
-            ex.sync();
-        }
-        // S5 update + warmstart, colour by colour
-        if (P.warmstart_coeff != 0.0f) {
-            for (int c = 0; c < ncol; ++c) {
-                int a = c0 + coff[c], e = c0 + coff[c + 1];
-                if (e > c1) e = c1;
-                if (a >= e) continue;
-                stage(a, e, c == ovf, MODE_WARMSTART, false);
-                ex.sync();
-            }
-        } else {
-            // warmstart_coefficient == 0: update only banks and zeroes the impulses (no velocity change)
-            for (int q = c0 + tid; q < c1; q += nth) {
-                if (grp && w.cons_key[q] != gk) continue;
-                Cons c;
-                cons_load<FM>(w, q, c);
-#pragma unroll
-                for (int k = 0; k < MAX_PTS; ++k)
-                    if (k < c.nc) { c.acc[k] = c.acc[k] + c.imp[k]; c.imp[k] = c.imp[k] * 0.0f; }
-                c.ta0 = c.ta0 + c.ti0; c.ta1 = c.ta1 + c.ti1; c.ti0 = c.ti0 * 0.0f; c.ti1 = c.ti1 * 0.0f;
-                c.wa = c.wa + c.wi; c.wi = c.wi * 0.0f;
-                if (FM) {
-#pragma unroll
-                    for (int k = 0; k < MAX_PTS; ++k)
-                        if (k < c.nc) {
-                            c.pta0[k] = c.pta0[k] + c.pti0[k]; c.pta1[k] = c.pta1[k] + c.pti1[k];
-                            c.pti0[k] = c.pti0[k] * 0.0f; c.pti1[k] = c.pti1[k] * 0.0f;
-                        }
-                }
-                cons_store_dyn<FM>(w, q, c);
-            }
-            ex.sync();
-        }
-        for (int pass = 0; pass < 2; ++pass) {
-            const bool relax = pass == 1;
-            const int iters = relax ? P.num_relax : P.num_pgs;
-            const bool fric = relax || P.friction_in_bias || P.num_relax == 0;
-            for (int it = 0; it < iters; ++it) {
-                const bool jwarm = JM && P.warmstart_joints && !relax && it == 0;   // fused into the first biased pass (worker.rs:548)
-                // joints first (solve.rs:89-92), then contacts
-                for (int c = 0; c < njcol; ++c) {
-                    int a = j0 + joff[c], e = j0 + joff[c + 1];
-                    if (a >= e) continue;
-                    if (c == jovf) {
-                        if (tid == 0) for (int q = a; q < e; ++q) { if (grp && w.j_key[q] != gk) continue; if (JM) joint_solve_generic(w, bd, q, relax, jwarm); else joint_solve(w, bd, q, relax); }
-                    } else {
-                        for (int q = a + tid; q < e; q += nth) { if (grp && w.j_key[q] != gk) continue; if (JM) joint_solve_generic(w, bd, q, relax, jwarm); else joint_solve(w, bd, q, relax); }
-                    }
-                    ex.sync();
-                }
-                for (int c = 0; c < ncol; ++c) {
-                    int a = c0 + coff[c], e = c0 + coff[c + 1];
-                    if (e > c1) e = c1;
-                    if (a >= e) continue;
-                    stage(a, e, c == ovf, relax ? MODE_RELAX : MODE_BIASED, fric);
-                    ex.sync();
-                }
-            }
-            if (!relax) {
-                for (int l = b0 + tid; l < b1; l += nth) {
-                    int b = w.item_bodies[l];
-                    if (grp && w.b_key[b] != gk) continue;
-                    body_integrate(w, bd, b, global_ids ? b : l - b0);
-                }
-                ex.sync();
-            }
-        }
-    }
-    // S9 restitution
-    if (w.item_flags[item]) {
-        for (int c = 0; c < ncol; ++c) {
-            int a = c0 + coff[c], e = c0 + coff[c + 1];
-            if (e > c1) e = c1;
-            if (a >= e) continue;
-            stage(a, e, c == ovf, MODE_RESTITUTION, false);
-            ex.sync();
-        }
-    }
-    // S10 impulse writeback
-    for (int q = c0 + tid; q < c1; q += nth) { if (grp && w.cons_key[q] != gk) continue; Cons cc; cons_load<FM>(w, q, cc); cons_writeback<FM>(w, q, buf, cc); }
-    for (int q = j0 + tid; q < j1; q += nth) { if (grp && w.j_key[q] != gk) continue; if (JM) joint_writeback_generic(w, q); else joint_writeback(w, q); }
-    for (int l = b0 + tid; l < b1; l += nth) {
-        int b = w.item_bodies[l];
-        if (grp && w.b_key[b] != gk) continue;
-        body_writeback(w, bd, b, global_ids ? b : l - b0);
-    }
-}
-
 // =====================================================================================================
 // Lane-cooperative shared-memory path: the island's bodies AND constraints live in shared memory for
 // the whole step; each constraint is swept by L consecutive lanes (L = 4 on the GPU: one lane per
@@ -1781,76 +1641,192 @@ RB_HD void coop_stage(const World& w, const B& bd, const RowView& cs, const RowV
     }
 }
 
-// The grid-wide "large" item 0 (islands too big for a CTA), lane-cooperative form: the same coop_stage as the
-// shared-memory items, with the constraint rows in the L2-resident World::large_pool / large_mut (row stride
-// cons_cap, indexed by schedule slot), the solver bodies in the global s_* tables (ids are body indices; the
-// world pseudo body is entry nb, the garbage slot nb + 1), and a grid barrier between colour stages.
-template <int L, class X, class B>
-RB_PHASE void solve_item_lanes(const X& ex, const World& w, const B& bd, vec3 gravity) {
-    const Params& P = w.prm;
-    State* st = w.st;
-    const int item = 0, buf = st->cur;
-    const int b0 = w.item_body_start[0], b1 = w.item_body_start[1];
-    const int c0 = w.item_cons_start[0];
-    const int c1 = w.item_cons_start[1] < w.cons_cap ? w.item_cons_start[1] : w.cons_cap;
-    const int j0 = w.item_joint_start[0], j1 = w.item_joint_start[1];
-    const int* coff = w.item_color_off;
-    const int* joff = w.item_jcolor_off;
-    const int ncol = st->nused_colors, njcol = st->njused_colors;
-    const int ovf = w.color_pos[COLOR_OVERFLOW], jovf = w.jcolor_pos[COLOR_OVERFLOW];
-    const int tid = ex.tid(), nth = ex.nth();
-    const int wslot = w.nb;
-    RowView rows, mu;
-    rows.p = w.large_pool; rows.stride = w.cons_cap;
-    mu.p = w.large_mut; mu.stride = w.cons_cap;
+// coop_stage for a sweep mode known only at run time.
+template <int L, class B>
+RB_HD void coop_stage_mode(int mode, const World& w, const B& bd, const RowView& cs, const RowView& mu, int wslot, int q0, int a, int e,
+                           int tid, int nth, bool solve_friction) {
+    if (mode == MODE_WARMSTART) coop_stage<L, MODE_WARMSTART>(w, bd, cs, mu, wslot, q0, a, e, tid, nth, solve_friction);
+    else if (mode == MODE_BIASED) coop_stage<L, MODE_BIASED>(w, bd, cs, mu, wslot, q0, a, e, tid, nth, solve_friction);
+    else if (mode == MODE_RELAX) coop_stage<L, MODE_RELAX>(w, bd, cs, mu, wslot, q0, a, e, tid, nth, solve_friction);
+    else coop_stage<L, MODE_RESTITUTION>(w, bd, cs, mu, wslot, q0, a, e, tid, nth, solve_friction);
+}
 
-    auto stage = [&](int a, int e, bool serial, int mode, bool fric) {
-        // the overflow colour is solved one constraint after the other by the first L lanes
-        const int t = tid, n = serial ? L : nth;
-        if (serial && tid >= L) return;
-        // stages with more constraints than lane groups are throughput-bound: one lane per constraint
-        // executes fewer instructions in total than L lanes sharing it
-        if (L > 1 && !serial && (e - a) * L > nth) {
-            if (mode == MODE_WARMSTART) coop_stage<1, MODE_WARMSTART>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-            else if (mode == MODE_BIASED) coop_stage<1, MODE_BIASED>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-            else if (mode == MODE_RELAX) coop_stage<1, MODE_RELAX>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-            else coop_stage<1, MODE_RESTITUTION>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-            return;
+// Bank the impulses of constraint s into their accumulators and scale them by `scale`: the warm-start
+// coefficient, or 0 when the step has no warm start (the impulses are then banked without being applied).
+RB_HD void coop_bank(const RowView& mu, int s, float scale) {
+    float4 im = mu.mr(MR_IMP, s), ac = mu.mr(MR_ACC, s), ti = mu.mr(MR_TI, s), wi = mu.mr(MR_WI, s);
+    ac.x = ac.x + im.x; ac.y = ac.y + im.y; ac.z = ac.z + im.z; ac.w = ac.w + im.w;
+    im.x = im.x * scale; im.y = im.y * scale; im.z = im.z * scale; im.w = im.w * scale;
+    ti.z = ti.z + ti.x; ti.w = ti.w + ti.y; ti.x = ti.x * scale; ti.y = ti.y * scale;
+    wi.y = wi.y + wi.x; wi.x = wi.x * scale;
+    mu.mr(MR_IMP, s) = im; mu.mr(MR_ACC, s) = ac; mu.mr(MR_TI, s) = ti; mu.mr(MR_WI, s) = wi;
+}
+
+// ---- the streaming / grid-wide solve ------------------------------------------------------------------
+// Constraint-row policies of solve_item: where a constraint's rows live between sweeps and which sweep reads them.
+//
+// HbmRows<FM, JM>: the Cons tables in HBM/L2, loaded, swept (cons_sweep) and stored back by one thread per
+// constraint.  The only rows with Coulomb friction (FM = 1) and generic joints (JM = 1).  generate / bank / writeback
+// work in the caller's Cons scratch `c` (see solve_item).
+template <int FM, int JM>
+struct HbmRows {
+    static constexpr bool solve_groups = true;   // a world with substep solve-groups takes these rows
+    static constexpr bool generic_joints = JM != 0;
+    RB_HD explicit HbmRows(const World&) {}
+    template <class B>
+    static RB_HD void begin(const World&, const B&) {}
+    template <class B>
+    static RB_HD void generate(const World& w, const B& bd, int q, int buf, int item, Cons& c) {
+        cons_generate<FM>(w, bd, q, buf, item, c);
+        cons_store_static<FM>(w, q, c);
+        cons_store_dyn<FM>(w, q, c);
+    }
+    // The constraints of colour stage [a, e) in the launch's solve-group: strided over the threads, or by thread 0 alone (serial).
+    template <class B>
+    static RB_HD void stage(const World& w, const B& bd, int a, int e, bool serial, int mode, bool fric, int tid, int nth, bool grp,
+                            unsigned char gk) {
+        if (serial) {
+            if (tid == 0)
+                for (int q = a; q < e; ++q) { if (grp && w.cons_key[q] != gk) continue; Cons cc; cons_load<FM>(w, q, cc); cons_sweep<FM>(w, bd, q, cc, mode, fric); cons_store_dyn<FM>(w, q, cc); }
+        } else {
+            for (int q = a + tid; q < e; q += nth) { if (grp && w.cons_key[q] != gk) continue; Cons cc; cons_load<FM>(w, q, cc); cons_sweep<FM>(w, bd, q, cc, mode, fric); cons_store_dyn<FM>(w, q, cc); }
         }
-        if (mode == MODE_WARMSTART) coop_stage<L, MODE_WARMSTART>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-        else if (mode == MODE_BIASED) coop_stage<L, MODE_BIASED>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-        else if (mode == MODE_RELAX) coop_stage<L, MODE_RELAX>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-        else coop_stage<L, MODE_RESTITUTION>(w, bd, rows, mu, wslot, 0, a, e, t, n, fric);
-    };
+    }
+    static RB_HD void bank(const World& w, int q, Cons& c) {   // bank and zero the impulses (no velocity change)
+        cons_load<FM>(w, q, c);
+#pragma unroll
+        for (int k = 0; k < MAX_PTS; ++k)
+            if (k < c.nc) { c.acc[k] = c.acc[k] + c.imp[k]; c.imp[k] = c.imp[k] * 0.0f; }
+        c.ta0 = c.ta0 + c.ti0; c.ta1 = c.ta1 + c.ti1; c.ti0 = c.ti0 * 0.0f; c.ti1 = c.ti1 * 0.0f;
+        c.wa = c.wa + c.wi; c.wi = c.wi * 0.0f;
+        if (FM) {
+#pragma unroll
+            for (int k = 0; k < MAX_PTS; ++k)
+                if (k < c.nc) {
+                    c.pta0[k] = c.pta0[k] + c.pti0[k]; c.pta1[k] = c.pta1[k] + c.pti1[k];
+                    c.pti0[k] = c.pti0[k] * 0.0f; c.pti1[k] = c.pti1[k] * 0.0f;
+                }
+        }
+        cons_store_dyn<FM>(w, q, c);
+    }
+    static RB_HD void writeback(const World& w, int q, int buf, Cons& c) { cons_load<FM>(w, q, c); cons_writeback<FM>(w, q, buf, c); }
+    template <class B>
+    static RB_HD void update_joint(const World& w, const B& bd, int q, int sub) { if (JM) joint_update_generic(w, bd, q, sub); else joint_update(w, bd, q); }
+    template <class B>   // warm: the generic joints' warm start, fused into the first biased pass (worker.rs:548)
+    static RB_HD void solve_joint(const World& w, const B& bd, int q, bool relax, bool warm) {
+        if (JM) joint_solve_generic(w, bd, q, relax, warm); else joint_solve(w, bd, q, relax);
+    }
+    static RB_HD void writeback_joint(const World& w, int q) { if (JM) joint_writeback_generic(w, q); else joint_writeback(w, q); }
+};
 
-    if (tid == 0) {
-        w.item_flags[item] = 0;
+// PoolRows<L>: the lane-cooperative rows of coop_stage (L lanes per constraint) in the L2-resident World::large_pool /
+// large_mut (row stride cons_cap, indexed by schedule slot).  For the grid-wide item 0 of the twist path: the solver
+// bodies are the global s_* tables (ids are body indices), the world pseudo body is entry nb, the garbage slot nb + 1.
+// No Coulomb friction, no generic joints and no substep solve-groups: a world with any of them takes HbmRows.
+template <int L>
+struct PoolRows {
+    static constexpr bool solve_groups = false;   // (the key filter costs k_collide and k_solve_large stack and spills)
+    static constexpr bool generic_joints = false;
+    RowView rows, mu;
+    int wslot;
+    RB_HD explicit PoolRows(const World& w) {
+        wslot = w.nb;
+        rows.p = w.large_pool; rows.stride = w.cons_cap;
+        mu.p = w.large_mut; mu.stride = w.cons_cap;
+    }
+    template <class B>
+    RB_HD void begin(const World& w, const B& bd) const {
         bd.set_vel(wslot, zero3(), zero3());
         bd.set_xf(wslot, pident());
         w.b_eim[wslot] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    for (int l = b0 + tid; l < b1; l += nth) {
-        int b = w.item_bodies[l];
-        body_init(w, bd, b, b, gravity);
-    }
-    ex.sync();
-    for (int q = c0 + tid; q < c1; q += nth) {   // S2 generate
-        Cons c;
+    template <class B>
+    RB_HD void generate(const World& w, const B& bd, int q, int buf, int item, Cons& c) const {
         cons_generate(w, bd, q, buf, item, c);
         coop_put(rows, mu, bd, q, c);
     }
+    template <class B>
+    RB_HD void stage(const World& w, const B& bd, int a, int e, bool serial, int mode, bool fric, int tid, int nth, bool, unsigned char) const {
+        // the overflow colour is solved one constraint after the other by the first L lanes
+        const int n = serial ? L : nth;
+        if (serial && tid >= L) return;
+        // stages with more constraints than lane groups are throughput-bound: one lane per constraint
+        // executes fewer instructions in total than L lanes sharing it
+        if (L > 1 && !serial && (e - a) * L > nth) coop_stage_mode<1>(mode, w, bd, rows, mu, wslot, 0, a, e, tid, n, fric);
+        else coop_stage_mode<L>(mode, w, bd, rows, mu, wslot, 0, a, e, tid, n, fric);
+    }
+    RB_HD void bank(const World&, int q, Cons&) const { coop_bank(mu, q, 0.0f); }
+    RB_HD void writeback(const World& w, int q, int buf, Cons& c) const {
+        coop_get_for_writeback(rows, mu, q, c);
+        cons_writeback(w, q, buf, c, true);
+    }
+    template <class B>
+    static RB_HD void update_joint(const World& w, const B& bd, int q, int) { joint_update(w, bd, q); }
+    template <class B>
+    static RB_HD void solve_joint(const World& w, const B& bd, int q, bool relax, bool) { joint_solve(w, bd, q, relax); }
+    static RB_HD void writeback_joint(const World& w, int q) { joint_writeback(w, q); }
+};
+
+// Solve one work item from solver-body init to the final positions of its bodies, with the constraint rows of policy R:
+// one CTA per item with its bodies in shared memory (BlockExec, SmemBodies), or the grid-wide item 0 with the bodies in
+// the global tables and grid barriers (GridExec / GridSpreadExec, GlobalBodies).
+template <class R, class X, class B>
+RB_PHASE void solve_item(const X& ex, const World& w, const B& bd, int item, vec3 gravity) {
+    const Params& P = w.prm;
+    State* st = w.st;
+    const int buf = st->cur;
+    const bool global_ids = item == 0;
+    const int b0 = w.item_body_start[item], b1 = w.item_body_start[item + 1];
+    const int c0 = w.item_cons_start[item];
+    const int c1 = w.item_cons_start[item + 1] < w.cons_cap ? w.item_cons_start[item + 1] : w.cons_cap;
+    const int j0 = w.item_joint_start[item], j1 = w.item_joint_start[item + 1];
+    const int* coff = w.item_color_off + (size_t)item * (NUM_COLORS + 1);
+    const int* joff = w.item_jcolor_off + (size_t)item * (NUM_COLORS + 1);
+    const int ncol = st->nused_colors, njcol = st->njused_colors;
+    const int ovf = w.color_pos[COLOR_OVERFLOW], jovf = w.jcolor_pos[COLOR_OVERFLOW];
+    const int tid = ex.tid(), nth = ex.nth();
+    // substep solve-groups: this launch solves the islands whose key is pass_key, at the cadence w.prm was derived for
+    const bool grp = R::solve_groups && w.any_extra != 0;
+    const unsigned char gk = (unsigned char)w.pass_key;
+    const R rows(w);
+
+    // The kernels of the general path sit at 255 registers with stack frames of 1-4 KB, and this function's shape decides
+    // them: the Cons scratch of generate / bank / writeback is declared by the loops here (not inside the policy), and the
+    // three colour-stage loops stay written out (not one lambda).  Either alternative costs those kernels 8-32 B of stack.
+    auto stage = [&](int a, int e, bool serial, int mode, bool fric) { rows.stage(w, bd, a, e, serial, mode, fric, tid, nth, grp, gk); };
+
+    if (tid == 0) {
+        w.item_flags[item] = 0;   // bit 0: some contact of this item holds a restitution seed
+        rows.begin(w, bd);
+    }
+    for (int l = b0 + tid; l < b1; l += nth) {
+        int b = w.item_bodies[l];
+        if (grp && w.b_key[b] != gk) continue;
+        body_init(w, bd, b, global_ids ? b : l - b0, gravity);
+    }
     ex.sync();
+    // S2 generate
+    for (int q = c0 + tid; q < c1; q += nth) {
+        if (grp && w.cons_key[q] != gk) continue;
+        Cons c;
+        rows.generate(w, bd, q, buf, item, c);
+    }
+    ex.sync();
+
     for (int sub = 0; sub < P.num_substeps; ++sub) {
         for (int l = b0 + tid; l < b1; l += nth) {
             int b = w.item_bodies[l];
-            body_increment(w, bd, b, b);
+            if (grp && w.b_key[b] != gk) continue;
+            body_increment(w, bd, b, global_ids ? b : l - b0);
         }
         ex.sync();
-        if (j1 > j0) {   // S4 joint rows from the current poses
-            for (int q = j0 + tid; q < j1; q += nth) joint_update(w, bd, q);
+        // S4 joint rows from the current poses
+        if (j1 > j0) {
+            for (int q = j0 + tid; q < j1; q += nth) { if (grp && w.j_key[q] != gk) continue; rows.update_joint(w, bd, q, sub); }
             ex.sync();
         }
-        if (P.warmstart_coeff != 0.0f) {   // S5 update + warmstart, colour by colour
+        // S5 update + warmstart, colour by colour
+        if (P.warmstart_coeff != 0.0f) {
             for (int c = 0; c < ncol; ++c) {
                 int a = c0 + coff[c], e = c0 + coff[c + 1];
                 if (e > c1) e = c1;
@@ -1858,14 +1834,12 @@ RB_PHASE void solve_item_lanes(const X& ex, const World& w, const B& bd, vec3 gr
                 stage(a, e, c == ovf, MODE_WARMSTART, false);
                 ex.sync();
             }
-        } else {   // warmstart_coefficient == 0: update only banks and zeroes the impulses
-            for (int s = c0 + tid; s < c1; s += nth) {
-                float4 im = mu.mr(MR_IMP, s), ac = mu.mr(MR_ACC, s), ti = mu.mr(MR_TI, s), wi = mu.mr(MR_WI, s);
-                ac.x = ac.x + im.x; ac.y = ac.y + im.y; ac.z = ac.z + im.z; ac.w = ac.w + im.w;
-                im.x = im.x * 0.0f; im.y = im.y * 0.0f; im.z = im.z * 0.0f; im.w = im.w * 0.0f;
-                ti.z = ti.z + ti.x; ti.w = ti.w + ti.y; ti.x = ti.x * 0.0f; ti.y = ti.y * 0.0f;
-                wi.y = wi.y + wi.x; wi.x = wi.x * 0.0f;
-                mu.mr(MR_IMP, s) = im; mu.mr(MR_ACC, s) = ac; mu.mr(MR_TI, s) = ti; mu.mr(MR_WI, s) = wi;
+        } else {
+            // warmstart_coefficient == 0: update only banks and zeroes the impulses (no velocity change)
+            for (int q = c0 + tid; q < c1; q += nth) {
+                if (grp && w.cons_key[q] != gk) continue;
+                Cons c;
+                rows.bank(w, q, c);
             }
             ex.sync();
         }
@@ -1874,13 +1848,15 @@ RB_PHASE void solve_item_lanes(const X& ex, const World& w, const B& bd, vec3 gr
             const int iters = relax ? P.num_relax : P.num_pgs;
             const bool fric = relax || P.friction_in_bias || P.num_relax == 0;
             for (int it = 0; it < iters; ++it) {
-                for (int c = 0; c < njcol; ++c) {   // joints first (solve.rs:89-92), then contacts
+                const bool jwarm = R::generic_joints && P.warmstart_joints && !relax && it == 0;   // fused into the first biased pass (worker.rs:548)
+                // joints first (solve.rs:89-92), then contacts
+                for (int c = 0; c < njcol; ++c) {
                     int a = j0 + joff[c], e = j0 + joff[c + 1];
                     if (a >= e) continue;
                     if (c == jovf) {
-                        if (tid == 0) for (int q = a; q < e; ++q) joint_solve(w, bd, q, relax);
+                        if (tid == 0) for (int q = a; q < e; ++q) { if (grp && w.j_key[q] != gk) continue; rows.solve_joint(w, bd, q, relax, jwarm); }
                     } else {
-                        for (int q = a + tid; q < e; q += nth) joint_solve(w, bd, q, relax);
+                        for (int q = a + tid; q < e; q += nth) { if (grp && w.j_key[q] != gk) continue; rows.solve_joint(w, bd, q, relax, jwarm); }
                     }
                     ex.sync();
                 }
@@ -1895,13 +1871,15 @@ RB_PHASE void solve_item_lanes(const X& ex, const World& w, const B& bd, vec3 gr
             if (!relax) {
                 for (int l = b0 + tid; l < b1; l += nth) {
                     int b = w.item_bodies[l];
-                    body_integrate(w, bd, b, b);
+                    if (grp && w.b_key[b] != gk) continue;
+                    body_integrate(w, bd, b, global_ids ? b : l - b0);
                 }
                 ex.sync();
             }
         }
     }
-    if (w.item_flags[item]) {   // S9 restitution
+    // S9 restitution
+    if (w.item_flags[item]) {
         for (int c = 0; c < ncol; ++c) {
             int a = c0 + coff[c], e = c0 + coff[c + 1];
             if (e > c1) e = c1;
@@ -1910,15 +1888,13 @@ RB_PHASE void solve_item_lanes(const X& ex, const World& w, const B& bd, vec3 gr
             ex.sync();
         }
     }
-    for (int q = c0 + tid; q < c1; q += nth) {   // S10 impulse writeback
-        Cons c;
-        coop_get_for_writeback(rows, mu, q, c);
-        cons_writeback(w, q, buf, c, true);
-    }
-    for (int q = j0 + tid; q < j1; q += nth) joint_writeback(w, q);
+    // S10 impulse writeback
+    for (int q = c0 + tid; q < c1; q += nth) { if (grp && w.cons_key[q] != gk) continue; Cons c; rows.writeback(w, q, buf, c); }
+    for (int q = j0 + tid; q < j1; q += nth) { if (grp && w.j_key[q] != gk) continue; rows.writeback_joint(w, q); }
     for (int l = b0 + tid; l < b1; l += nth) {
         int b = w.item_bodies[l];
-        body_writeback(w, bd, b, b);
+        if (grp && w.b_key[b] != gk) continue;
+        body_writeback(w, bd, b, global_ids ? b : l - b0);
     }
 }
 
@@ -2014,12 +1990,7 @@ RB_PHASE void coop_sweep(const BlockCtx& ctx, const World& w, const SmemBodies& 
 // Walking each body's adjacency list (slot order = colour order, built by the schedule) reproduces exactly
 // that sequence -- same operands, same order, same bits -- with one barrier instead of one per colour.
 RB_HD void coop_warmstart_bank(const Params& P, const RowView& mu, int s) {   // the per-constraint half: bank and scale
-    float4 im = mu.mr(MR_IMP, s), ac = mu.mr(MR_ACC, s), ti = mu.mr(MR_TI, s), wi = mu.mr(MR_WI, s);
-    ac.x = ac.x + im.x; ac.y = ac.y + im.y; ac.z = ac.z + im.z; ac.w = ac.w + im.w;
-    im.x = im.x * P.warmstart_coeff; im.y = im.y * P.warmstart_coeff; im.z = im.z * P.warmstart_coeff; im.w = im.w * P.warmstart_coeff;
-    ti.z = ti.z + ti.x; ti.w = ti.w + ti.y; ti.x = ti.x * P.warmstart_coeff; ti.y = ti.y * P.warmstart_coeff;
-    wi.y = wi.y + wi.x; wi.x = wi.x * P.warmstart_coeff;
-    mu.mr(MR_IMP, s) = im; mu.mr(MR_ACC, s) = ac; mu.mr(MR_TI, s) = ti; mu.mr(MR_WI, s) = wi;
+    coop_bank(mu, s, P.warmstart_coeff);
 }
 // One side of one constraint applied to its body (v, wv): the operations coop_stage<MODE_WARMSTART> performs on that side.
 RB_HD void coop_warmstart_side(const RowView& cs, const RowView& mu, int s, int side, vec3 im, vec3& v, vec3& wv) {
@@ -2092,8 +2063,7 @@ RB_PHASE void solve_item_coop(const BlockCtx& ctx, const World& w, float* smem, 
         // of the CTA only help with generation, integration and writeback (fewer warps = shorter issue queues)
         int longest = 0;
         for (int c = 0; c < ns; ++c) longest = max2i(longest, (s_stage[c] >> 16) - (s_stage[c] & 0xffff));
-        int width = (longest * L + 31) & ~31;
-        if (w.coop_sweep_threads > 0) width = w.coop_sweep_threads;
+        const int width = (longest * L + 31) & ~31;
         s_width = min2i(nth, max2i(width, 128));
         int nq = 0;
         if (!resident)
@@ -2163,14 +2133,7 @@ RB_PHASE void solve_item_coop(const BlockCtx& ctx, const World& w, float* smem, 
             ctx.block_sync();
             if (sub == 0) RB_TRACE();
         } else {   // bank the impulses without applying them
-            for (int s = tid; s < n; s += nth) {
-                float4 im = mu.mr(MR_IMP, s), ac = mu.mr(MR_ACC, s), ti = mu.mr(MR_TI, s), wi = mu.mr(MR_WI, s);
-                ac.x = ac.x + im.x; ac.y = ac.y + im.y; ac.z = ac.z + im.z; ac.w = ac.w + im.w;
-                im.x = im.x * 0.0f; im.y = im.y * 0.0f; im.z = im.z * 0.0f; im.w = im.w * 0.0f;
-                ti.z = ti.z + ti.x; ti.w = ti.w + ti.y; ti.x = ti.x * 0.0f; ti.y = ti.y * 0.0f;
-                wi.y = wi.y + wi.x; wi.x = wi.x * 0.0f;
-                mu.mr(MR_IMP, s) = im; mu.mr(MR_ACC, s) = ac; mu.mr(MR_TI, s) = ti; mu.mr(MR_WI, s) = wi;
-            }
+            for (int s = tid; s < n; s += nth) coop_bank(mu, s, 0.0f);
             ctx.block_sync();
         }
         for (int pass = 0; pass < 2; ++pass) {

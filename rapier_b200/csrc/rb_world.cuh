@@ -258,7 +258,6 @@ struct World {
     int coop_small_floats;            // dynamic shared memory of the small launch shape (2 CTAs / SM), which must fit every shared-memory item
     long long* dbg_times;             // [32] phase timestamps of one item (debug_flags & 2)
     int debug_flags;                  // RB_DEBUG_FLAGS, honoured only by the -DRB_DEBUG build: 1 = skip the sweeps, 2 = record dbg_times
-    int coop_sweep_threads;           // sweep width of the big launch shape (0 = whole block)
     int* host_hint;                   // pinned, host-mapped words read by the host without synchronising: [0] last step's State::need_big,
                                       // [1] first status raised on the device since the host last cleared it (RbStatus; 0 = none)
                                       // [2] a grid-wide island exists, [3] CCD clamps are queued (applied by the next k_collide or synchronising call)
@@ -270,7 +269,7 @@ struct World {
     float4* j_rows;                   // [JR_ROWS][6 * joint_cap] per-substep rows
     int4* j_sched_ids;                // [joint_cap] joint, id1, id2, nrows in schedule order
     // limits and motors of the free axes (JointLimits / JointMotor, generic_joint.rs:142-232): only worlds in which some joint
-    // has any take the generic joint path (solve_item<FM, 1>, 12 row slots per joint instead of 6)
+    // has any take the generic joint path (solve_item<HbmRows<FM, 1>>, 12 row slots per joint instead of 6)
     int generic_joints;
     // Substep solve-groups (RigidBody::additional_solver_iterations; island_manager/substep_groups.rs): any_extra = some
     // body asks for extra substeps.  Then every island carries a key (max over its members, isl_key), the general solve
