@@ -1923,7 +1923,6 @@ struct CoopPipe {
     int nchunks;
     unsigned t;
     int sweep_threads;          // threads that take part in the sweeps (a multiple of the warp size, <= block size)
-    bool primed;                // the chunk the next sweep starts with is already in flight
 };
 RB_HD RowView coop_chunk_rows(const CoopPipe& pp, int q) {   // pool rows of chunk q, indexed by item slot
     const int o = pp.chunk[q], cnt = pp.chunk[q + 1] - o;
@@ -1948,7 +1947,8 @@ RB_HD void coop_pipe_issue(const CoopPipe& pp, int q, int b) {   // one thread: 
 }
 
 // One sweep over all colour stages of the item.  Resident items read their shared-memory rows; streamed
-// items consume the pipeline.  `wrap`: another sweep follows, its first chunk is prefetched by the last one here.
+// items consume the pipeline, whose first chunk is already in flight (issued after generate, or by the sweep
+// before).  `wrap`: another sweep follows, its first chunk is prefetched by the last one here.
 template <int L, int MODE>
 RB_PHASE void coop_sweep(const BlockCtx& ctx, const World& w, const SmemBodies& bd, const RowView& res, const RowView& mu, bool resident,
                          CoopPipe& pp, const int* s_stage, int nstages, int wslot, int c0, bool fric, bool wrap) {
@@ -1964,7 +1964,6 @@ RB_PHASE void coop_sweep(const BlockCtx& ctx, const World& w, const SmemBodies& 
         }
         return;
     }
-    if (!pp.primed && tid == 0) coop_pipe_issue(pp, 0, pp.t & 1);   // (the caller synchronised after the rows were written and fenced)
     for (int q = 0; q < pp.nchunks; ++q) {
         const int o = pp.chunk[q], e = pp.chunk[q + 1];
         const int b = pp.t & 1;
@@ -1980,7 +1979,6 @@ RB_PHASE void coop_sweep(const BlockCtx& ctx, const World& w, const SmemBodies& 
         ctx.block_sync();
         pp.t += 1;
     }
-    pp.primed = wrap;
 }
 
 // ---- warm start of a shared-memory item, body-centric ------------------------------------------------
@@ -1989,36 +1987,49 @@ RB_PHASE void coop_sweep(const BlockCtx& ctx, const World& w, const SmemBodies& 
 // constraint, so what a body ends up with is the sequence of additions of ITS constraints in colour order.
 // Walking each body's adjacency list (slot order = colour order, built by the schedule) reproduces exactly
 // that sequence -- same operands, same order, same bits -- with one barrier instead of one per colour.
+// Streamed items gather the same way, reading the constant rows from the L2 pool instead of shared memory.
 RB_HD void coop_warmstart_bank(const Params& P, const RowView& mu, int s) {   // the per-constraint half: bank and scale
     coop_bank(mu, s, P.warmstart_coeff);
 }
+// The rows one side of constraint s adds to its body in the warm start, loaded apart from their use so that a
+// body's gather can fetch the next constraint's rows (L2 latency for a streamed item) while it applies the
+// current one.  The rows of points beyond nc are loaded too (generate writes every point row) and never used.
+struct WarmSide { float4 dirf, t1w, trn, itd[MAX_PTS], jac[5], imp, ti, wi; };
+RB_HD WarmSide coop_warmstart_load(const RowView& cs, const RowView& mu, int s, int side) {
+    WarmSide o;
+    o.dirf = cs.pc(CR4_DIRF, s); o.t1w = cs.pc(CR4_T1W, s); o.trn = cs.pc(CR4_TR, s);
+#pragma unroll
+    for (int k = 0; k < MAX_PTS; ++k) o.itd[k] = cs.pp(side == 0 ? PR4_ITD1I : PR4_ITD2A, k, s);
+#pragma unroll
+    for (int r = 0; r < 5; ++r) o.jac[r] = cs.pc(CR4_J3 + r, s);   // i10 i11 i20 i21 tw1 tw2 (see coop_put_jac)
+    o.imp = mu.mr(MR_IMP, s); o.ti = mu.mr(MR_TI, s); o.wi = mu.mr(MR_WI, s);
+    return o;
+}
 // One side of one constraint applied to its body (v, wv): the operations coop_stage<MODE_WARMSTART> performs on that side.
-RB_HD void coop_warmstart_side(const RowView& cs, const RowView& mu, int s, int side, vec3 im, vec3& v, vec3& wv) {
-    const float4 dirf = cs.pc(CR4_DIRF, s), t1w = cs.pc(CR4_T1W, s), trn = cs.pc(CR4_TR, s);
-    const float4 imp4 = mu.mr(MR_IMP, s), ti4 = mu.mr(MR_TI, s), wi4 = mu.mr(MR_WI, s);
-    const int nc = as_int(trn.w);
-    const vec3 dir = xyz(dirf), t1 = xyz(t1w);
+RB_HD void coop_warmstart_apply(const WarmSide& o, int side, vec3 im, vec3& v, vec3& wv) {
+    const int nc = as_int(o.trn.w);
+    const vec3 dir = xyz(o.dirf), t1 = xyz(o.t1w);
     const vec3 t2 = cross3(dir, t1);
     const vec3 lin = had(dir, im);
-    const float imp[MAX_PTS] = {imp4.x, imp4.y, imp4.z, imp4.w};
+    const float imp[MAX_PTS] = {o.imp.x, o.imp.y, o.imp.z, o.imp.w};
 #pragma unroll
     for (int k = 0; k < MAX_PTS; ++k) {
         if (k < nc) {
-            const vec3 itd = xyz(cs.pp(side == 0 ? PR4_ITD1I : PR4_ITD2A, k, s));
+            const vec3 itd = xyz(o.itd[k]);
             v = madd3(v, lin, side == 0 ? imp[k] : -imp[k]);
             wv = madd3(wv, itd, imp[k]);
         }
     }
-    const FrictionJac j = coop_get_jac(cs, s);
-    const float ti0 = ti4.x, ti1 = ti4.y, wi = wi4.x;
+    const float4 d = o.jac[0], e = o.jac[1], f = o.jac[2], g = o.jac[3], h = o.jac[4];
+    const float ti0 = o.ti.x, ti1 = o.ti.y, wi = o.wi.x;
     if (side == 0) {
         v = madd3v(v, madd3(t1 * ti0, t2, ti1), im);
-        wv = madd3(madd3(wv, j.i10, ti0), j.i11, ti1);
-        if (nc > 1) wv = madd3(wv, j.tw1, wi);
+        wv = madd3(madd3(wv, mk3(d.x, d.y, d.z), ti0), mk3(d.w, e.x, e.y), ti1);
+        if (nc > 1) wv = madd3(wv, mk3(g.x, g.y, g.z), wi);
     } else {
         v = madd3v(v, madd3(t1 * (-ti0), t2, -ti1), im);
-        wv = madd3(madd3(wv, j.i20, ti0), j.i21, ti1);
-        if (nc > 1) wv = madd3(wv, j.tw2, -wi);
+        wv = madd3(madd3(wv, mk3(e.z, e.w, f.x), ti0), mk3(f.y, f.z, f.w), ti1);
+        if (nc > 1) wv = madd3(wv, mk3(g.w, h.x, h.y), -wi);
     }
 }
 
@@ -2051,7 +2062,7 @@ RB_PHASE void solve_item_coop(const BlockCtx& ctx, const World& w, float* smem, 
     RB_SHARED int s_nchunks;
     RB_SHARED int s_width;
     pp.buf[0] = cbase; pp.buf[1] = cbase + (size_t)COOP_ROWS * plan.stride;
-    pp.pool = w.coop_pool + (size_t)2 * COOP_ROWS * c0; pp.chunk = s_chunk; pp.primed = false;
+    pp.pool = w.coop_pool + (size_t)2 * COOP_ROWS * c0; pp.chunk = s_chunk;
     if (tid == 0) {
         const int* coff = w.item_color_off + (size_t)item * (NUM_COLORS + 1);
         const int ncol = st->nused_colors;
@@ -2102,17 +2113,17 @@ RB_PHASE void solve_item_coop(const BlockCtx& ctx, const World& w, float* smem, 
     RB_TRACE();
     const bool bouncy_item = w.item_flags[item] != 0;
     const bool warm = P.warmstart_coeff != 0.0f;
-    const int total_sweeps = P.num_substeps * ((warm ? 1 : 0) + P.num_pgs + P.num_relax) + (bouncy_item ? 1 : 0);   // (pipeline sweeps of a streamed item)
+    // The pipeline sweeps of a streamed item.  The first chunk of the first one is staged from here on: nothing
+    // before that sweep reads the staging buffers (the warm start reads the rows from the pool).
+    int total_sweeps = P.num_substeps * (P.num_pgs + P.num_relax) + (bouncy_item ? 1 : 0);
+#ifdef RB_DEBUG
+    if (w.debug_flags & 1) total_sweeps = 0;   // (the sweeps are skipped: no chunk may be left in flight)
+#endif
+    if (!resident && total_sweeps > 0 && tid == 0) coop_pipe_issue(pp, 0, pp.t & 1);
     int done = 0;
     for (int sub = 0; sub < P.num_substeps; ++sub) {
         for (int l = b0 + tid; l < b1; l += nth) body_increment(w, bd, w.item_bodies[l], l - b0);
-        if (warm && !resident) {   // streamed rows: warm start colour by colour through the staging pipeline
-            ctx.block_sync();
-            ++done;
-            if (sub == 0) RB_TRACE();
-            coop_sweep<L, MODE_WARMSTART>(ctx, w, bd, res, mu, resident, pp, s_stage, nstages, wslot, c0, false, done < total_sweeps);
-            if (sub == 0) RB_TRACE();
-        } else if (warm) {         // resident rows: body-centric (one barrier instead of one per colour)
+        if (warm) {   // body-centric (one barrier instead of one per colour)
             if (sub == 0) RB_TRACE();
             for (int s = tid; s < n; s += nth) coop_warmstart_bank(P, mu, s);
             ctx.block_sync();   // (also orders the increments above before the gathers below)
@@ -2124,9 +2135,20 @@ RB_PHASE void solve_item_coop(const BlockCtx& ctx, const World& w, float* smem, 
                     const int cnt = w.adj_cnt[b0 + l];
                     vec3 v = bd.lin(l), wv = bd.ang(l);
                     const vec3 im = bd.im(l);
-                    for (int i = 0; i < cnt; ++i) {
-                        const int e = adj[i];
-                        coop_warmstart_side(res, mu, e >> 1, e & 1, im, v, wv);
+                    if (cnt > 0) {
+                        // software pipeline: the rows of entry i + 1 and list entry i + 2 are in flight while entry i is applied
+                        int e = adj[0], e_after = cnt > 1 ? adj[1] : 0;
+                        WarmSide next = coop_warmstart_load(resident ? res : coop_slot_rows(pp, e >> 1), mu, e >> 1, e & 1);
+                        for (int i = 0; i < cnt; ++i) {
+                            const WarmSide cur = next;
+                            const int side = e & 1;
+                            if (i + 1 < cnt) {
+                                e = e_after;
+                                if (i + 2 < cnt) e_after = adj[i + 2];
+                                next = coop_warmstart_load(resident ? res : coop_slot_rows(pp, e >> 1), mu, e >> 1, e & 1);
+                            }
+                            coop_warmstart_apply(cur, side, im, v, wv);
+                        }
                     }
                     bd.set_vel(l, v, wv);
                 }
