@@ -9,8 +9,11 @@
 //                   chain fused; constant constraint rows resident or streamed from L2 by bulk (TMA) copies
 // All sizes that change at run time (pairs, manifolds, items) live in device memory (rb::State).
 //
-// With -DRB_EMULATE (tests/emul only) the same phase functions run single-threaded on the host with
-// malloc'd tables: a logic check for machines without a GPU, never part of the product library.
+// With -DRB_EMULATE (tests/emul only) the same kernels and the same host code run on the host with malloc'd
+// tables: launch() calls each kernel as one CTA of one thread.  A logic check of the kernels and of the
+// step's launch sequence for machines without a GPU, never part of the product library.  It differs from
+// the device in two places: the 4-lane kernels run 1 lane per constraint (CONS_LANES), and
+// RB_EMU_COOP_SMEM_FLOATS can lower the shared-memory budget of both k_solve_coop launch shapes.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -46,6 +49,10 @@ static cudaError_t dev_free(void* p) { return cudaFree(p); }
 static cudaError_t h2d(void* d, const void* h, size_t n) { return n ? cudaMemcpy(d, h, n, cudaMemcpyHostToDevice) : cudaSuccess; }
 static cudaError_t d2h(void* h, const void* d, size_t n) { return n ? cudaMemcpy(h, d, n, cudaMemcpyDeviceToHost) : cudaSuccess; }
 static cudaError_t dev_set(void* d, int v, size_t n) { return n ? cudaMemset(d, v, n) : cudaSuccess; }
+static cudaError_t set_device(int d) { return cudaSetDevice(d); }
+static cudaError_t stream_sync(cudaStream_t s) { return cudaStreamSynchronize(s); }
+static cudaError_t memset_async(void* d, int v, size_t n, cudaStream_t s) { return cudaMemsetAsync(d, v, n, s); }
+static cudaError_t copy_async(void* d, const void* h, size_t n, cudaMemcpyKind k, cudaStream_t s) { return cudaMemcpyAsync(d, h, n, k, s); }
 #else
 #define CK(call)                                 \
     do {                                         \
@@ -56,6 +63,10 @@ static cudaError_t dev_free(void* p) { free(p); return cudaSuccess; }
 static cudaError_t h2d(void* d, const void* h, size_t n) { if (n) memcpy(d, h, n); return cudaSuccess; }
 static cudaError_t d2h(void* h, const void* d, size_t n) { if (n) memcpy(h, d, n); return cudaSuccess; }
 static cudaError_t dev_set(void* d, int v, size_t n) { if (n) memset(d, v, n); return cudaSuccess; }
+static cudaError_t set_device(int) { return cudaSuccess; }
+static cudaError_t stream_sync(cudaStream_t) { return cudaSuccess; }
+static cudaError_t memset_async(void* d, int v, size_t n, cudaStream_t) { return dev_set(d, v, n); }
+static cudaError_t copy_async(void* d, const void* h, size_t n, cudaMemcpyKind, cudaStream_t) { return h2d(d, h, n); }
 #endif
 
 // ------------------------------------------------------------------------------------------------
@@ -68,6 +79,9 @@ constexpr int ITEM_SMEM_BYTES = ITEM_MAX_BODIES * SB_STRIDE * 4;
 // constraints are streamed from the L2 pool, or that only fit resident here).
 constexpr int COOP_SMALL_THREADS = 128, COOP_SMALL_SMEM_BYTES = 108 * 1024;
 constexpr int COOP_BIG_THREADS = 256, COOP_BIG_SMEM_BYTES = 220 * 1024;
+// Lanes per constraint of the lane-cooperative kernels (k_collide's inline item-0 solve, k_solve_large, k_solve_coop).
+// The emulation's one thread has no lane groups: it runs them with one lane.
+constexpr int CONS_LANES = RB_DEVICE_BUILD ? 4 : 1;
 
 struct Grav { float x, y, z; };
 
@@ -232,7 +246,6 @@ RB_PHASE void set_halo_phase(const Ctx& ctx, const World& w, const unsigned char
     }
 }
 
-#if RB_DEVICE_BUILD
 // Collision pipeline, then every solve that is NOT shared-memory resident: work items streamed from
 // HBM (one CTA each) and the grid-wide "large" item 0.  Those touch bodies / constraints disjoint from
 // the items k_solve_coop handles next, so the order between the two kernels does not matter.
@@ -240,8 +253,8 @@ RB_PHASE void set_halo_phase(const Ctx& ctx, const World& w, const unsigned char
 // bit 1 set: k_solve_large follows and solves the grid-wide item 0.
 // SHAPES = 1: the variant for worlds with capsules (rb_geom.cuh); the ball / cuboid kernel is SHAPES = 0.
 template <int SHAPES>
-__global__ void __launch_bounds__(COLLIDE_THREADS) k_collide(World w, Grav g, int do_solve) {
-    extern __shared__ __align__(16) float smem[];
+RB_KERNEL RB_BOUNDS(COLLIDE_THREADS) k_collide(World w, Grav g, int do_solve) {
+    RB_DYNAMIC_SMEM(smem);
     GridCtx ctx;
     if (ctx.gtid == 0) {   // publish last step's launch hints to the host (read without synchronising)
         w.host_hint[0] = w.st->need_big;
@@ -273,13 +286,13 @@ __global__ void __launch_bounds__(COLLIDE_THREADS) k_collide(World w, Grav g, in
         bd.s = smem;
         BlockExec ex;
         ex.c = &bctx;
-        __shared__ int s_next;
+        RB_SHARED int s_next;
         const int n = w.st->norder;
         for (;;) {   // items that are not shared-memory items, most expensive first
-            if (bctx.btid == 0) s_next = atomicAdd(&w.st->cursor_rest, 1);
-            __syncthreads();
+            if (bctx.btid == 0) s_next = atomic_add(&w.st->cursor_rest, 1);
+            bctx.block_sync();
             const int k = s_next;
-            __syncthreads();
+            bctx.block_sync();
             if (k >= n) break;
             const int item = w.item_order[k];
             if (item_is_coop(w, item)) continue;
@@ -295,19 +308,19 @@ __global__ void __launch_bounds__(COLLIDE_THREADS) k_collide(World w, Grav g, in
     gb.w = &w;
     GridSpreadExec gex;
     gex.c = &ctx;
-    solve_item<PoolRows<4>>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
+    solve_item<PoolRows<CONS_LANES>>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
 }
 // The grid-wide item 0: islands too large for one CTA (pyramid3, keva3, joint grids).  Cooperative, one CTA per SM;
 // bodies in the global solver-body tables, constant rows in the L2-resident large pool, one grid barrier per colour
 // stage; consecutive warps of a stage's constraints go to different SMs (GridSpreadExec).
-__global__ void __launch_bounds__(COLLIDE_THREADS, 1) k_solve_large(World w, Grav g) {
+RB_KERNEL RB_BOUNDS(COLLIDE_THREADS, 1) k_solve_large(World w, Grav g) {
     GridCtx ctx;
     if (w.st->nlarge_bodies == 0) return;
     GlobalBodies gb;
     gb.w = &w;
     GridSpreadExec gex;
     gex.c = &ctx;
-    solve_item<PoolRows<4>>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
+    solve_item<PoolRows<CONS_LANES>>(gex, w, gb, 0, mk3(g.x, g.y, g.z));
 }
 // The general solve path, compiled per (friction model FM, joint model JM):
 //   FM = 1  FrictionModel::Coulomb (integration_parameters.rs:26-29): one coupled tangent part per contact point
@@ -315,27 +328,27 @@ __global__ void __launch_bounds__(COLLIDE_THREADS, 1) k_solve_large(World w, Gra
 // Every work item takes the streaming solve (solve_item<HbmRows<FM, JM>>: bodies in shared memory, rows in HBM/L2), the
 // grid-wide item 0 the same code with grid barriers.  The twist / locked-axes kernels carry none of this code.
 template <int FM, int JM>
-__global__ void __launch_bounds__(COLLIDE_THREADS) k_solve_items_x(World w, Grav g) {
-    extern __shared__ __align__(16) float smem[];
+RB_KERNEL RB_BOUNDS(COLLIDE_THREADS) k_solve_items_x(World w, Grav g) {
+    RB_DYNAMIC_SMEM(smem);
     BlockCtx bctx;
     SmemBodies bd;
     bd.s = smem;
     BlockExec ex;
     ex.c = &bctx;
-    __shared__ int s_next;
+    RB_SHARED int s_next;
     const int n = w.st->norder;
     for (;;) {
-        if (bctx.btid == 0) s_next = atomicAdd(&w.st->cursor_rest, 1);
-        __syncthreads();
+        if (bctx.btid == 0) s_next = atomic_add(&w.st->cursor_rest, 1);
+        bctx.block_sync();
         const int k = s_next;
-        __syncthreads();
+        bctx.block_sync();
         if (k >= n) break;
         solve_item<HbmRows<FM, JM>>(ex, w, bd, w.item_order[k], mk3(g.x, g.y, g.z));
         ex.sync();
     }
 }
 template <int FM, int JM>
-__global__ void __launch_bounds__(COLLIDE_THREADS, 1) k_solve_large_x(World w, Grav g) {
+RB_KERNEL RB_BOUNDS(COLLIDE_THREADS, 1) k_solve_large_x(World w, Grav g) {
     GridCtx ctx;
     if (w.st->nlarge_bodies == 0) return;
     GlobalBodies gb;
@@ -349,9 +362,9 @@ __global__ void __launch_bounds__(COLLIDE_THREADS, 1) k_solve_large_x(World w, G
 // Either launch shape takes every shared-memory item (the small one streams what does not fit), so the
 // host's choice between them -- a hint read without synchronising -- only affects speed.
 template <int L>
-__device__ __forceinline__ void solve_coop_items(const World& w, const Grav& g, int smem_floats) {
-    extern __shared__ __align__(16) float smem[];
-    __shared__ __align__(8) unsigned long long s_mbar[2];
+RB_D void solve_coop_items(const World& w, const Grav& g, int smem_floats) {
+    RB_DYNAMIC_SMEM(smem);
+    RB_SHARED __align__(8) unsigned long long s_mbar[2];
     BlockCtx ctx;
     if (ctx.btid == 0) {
         mbar_init(&s_mbar[0], 1);
@@ -363,33 +376,33 @@ __device__ __forceinline__ void solve_coop_items(const World& w, const Grav& g, 
     pp.mbar = s_mbar;
     pp.t = 0;
     pp.sweep_threads = ctx.bsize;   // (set per item)
-    __shared__ int s_next;
+    RB_SHARED int s_next;
     const int n = w.st->norder;
     int* cursor = &w.st->cursor_coop;
     for (;;) {   // dynamic queue over the cost-ordered items
-        if (ctx.btid == 0) s_next = atomicAdd(cursor, 1);
-        __syncthreads();
+        if (ctx.btid == 0) s_next = atomic_add(cursor, 1);
+        ctx.block_sync();
         const int k = s_next;
-        __syncthreads();
+        ctx.block_sync();
         if (k >= n) break;
         const int item = w.item_order[k];
         if (!item_is_coop(w, item)) continue;
-        solve_item_coop<L>(ctx, w, smem, smem_floats, pp, item, mk3(g.x, g.y, g.z));
+        solve_item_coop<L>(ctx, w, smem, smem_budget(smem_floats), pp, item, mk3(g.x, g.y, g.z));
         ctx.block_sync();
     }
 }
 // The two launch shapes (COOP_SMALL_* / COOP_BIG_*): same code, different register budgets.
-__global__ void __launch_bounds__(COOP_SMALL_THREADS, 2) k_solve_coop(World w, Grav g) { solve_coop_items<4>(w, g, COOP_SMALL_SMEM_BYTES / 4); }
-__global__ void __launch_bounds__(COOP_BIG_THREADS, 1) k_solve_coop_big(World w, Grav g) { solve_coop_items<1>(w, g, COOP_BIG_SMEM_BYTES / 4); }
-__global__ void k_kat(World w, int which, const float* in, float* out) { kat_phase(w, which, in, out); }
+RB_KERNEL RB_BOUNDS(COOP_SMALL_THREADS, 2) k_solve_coop(World w, Grav g) { solve_coop_items<CONS_LANES>(w, g, COOP_SMALL_SMEM_BYTES / 4); }
+RB_KERNEL RB_BOUNDS(COOP_BIG_THREADS, 1) k_solve_coop_big(World w, Grav g) { solve_coop_items<1>(w, g, COOP_BIG_SMEM_BYTES / 4); }
+RB_KERNEL k_kat(World w, int which, const float* in, float* out) { kat_phase(w, which, in, out); }
 // Contact force events of the step just solved (launched only for worlds in which a collider asks for them).
-__global__ void k_force_events(World w) {
+RB_KERNEL k_force_events(World w) {
     GridCtx ctx;
     phase_force_events(ctx, w);
 }
 // The CCD clamps queued by the last step's body writeback (rb_solver.cuh) when NO further step follows: a synchronising
 // call launches this (one CTA: fast bodies are rare) if the device flagged any; otherwise the next k_collide applies them.
-__global__ void k_ccd_pending(World w) {
+RB_KERNEL k_ccd_pending(World w) {
     GridCtx ctx;
     const int n = w.st->nccd;
     if (n == 0) return;
@@ -397,35 +410,34 @@ __global__ void k_ccd_pending(World w) {
 #pragma unroll 1
     for (int pass = 0; pass < npass; ++pass) {
         phase_ccd_pending(ctx, w, n, pass == 1);
-        __syncthreads();
+        ctx.block_sync();
     }
     if (ctx.gtid == 0) { w.st->nccd = 0; w.st->nccd_bullets = 0; w.host_hint[3] = 0; }
 }
-__global__ void k_init_bodies(World w, int first) {
+RB_KERNEL k_init_bodies(World w, int first) {
     GridCtx ctx;
     init_bodies_phase(ctx, w, first);
 }
-__global__ void k_wake(World w, const int* idx, int n) {
+RB_KERNEL k_wake(World w, const int* idx, int n) {
     GridCtx ctx;
     wake_phase(ctx, w, idx, n);
 }
-__global__ void k_wake_apply(World w) {
+RB_KERNEL k_wake_apply(World w) {
     GridCtx ctx;
     wake_apply_phase(ctx, w);
 }
-__global__ void k_import_halo(World w) {
+RB_KERNEL k_import_halo(World w) {
     GridCtx ctx;
     import_halo_phase(ctx, w);
 }
-__global__ void k_set_halo(World w, const unsigned char* flags) {
+RB_KERNEL k_set_halo(World w, const unsigned char* flags) {
     GridCtx ctx;
     set_halo_phase(ctx, w, flags);
 }
-__global__ void k_import_states(World w, const int* idx, const float* src, int n, int table) {
+RB_KERNEL k_import_states(World w, const int* idx, const float* src, int n, int table) {
     GridCtx ctx;
     import_states_phase(ctx, w, idx, src, n, table);
 }
-#endif
 
 // ------------------------------------------------------------------------------------------------
 // host-side world
@@ -462,16 +474,40 @@ struct RbWorld {
     float* stage_dev = nullptr;      // [nb*13] device staging for bulk state import
     int* ident_dev = nullptr;        // [nb] identity index list
     float* stage_host = nullptr;     // pinned host staging (2 * nb * 13 floats: in, out)
+    cudaStream_t stream = nullptr;   // (the emulation has none)
 #if RB_DEVICE_BUILD
-    cudaStream_t stream = nullptr;
     bool own_stream = true;
     std::vector<cudaEvent_t> prof_ev;   // 3 events per profiled step
     int prof_steps = 0;
 #else
-    std::vector<float> emu_smem;
-    int emu_coop_floats = 0, emu_hint[4] = {0, 0, 0, 0};
+    std::vector<float> emu_smem;   // dynamic shared memory of the emulated kernels
+    int emu_coop_floats = COOP_BIG_SMEM_BYTES / 4, emu_hint[4] = {0, 0, 0, 0};
 #endif
 };
+
+template <class T> struct same_type { using type = T; };
+// Launches `kernel` on the world's stream and counts it.  The emulation calls it as one CTA of one thread, with
+// `smem_bytes` of host memory as its dynamic shared memory, of which it may plan with at most emu_coop_floats.
+template <class... P>
+static cudaError_t launch(RbWorld* W, void (*kernel)(P...), int grid, int block, size_t smem_bytes, bool cooperative,
+                          typename same_type<P>::type... args) {
+#if RB_DEVICE_BUILD
+    void* argv[] = {(void*)&args...};
+    const cudaError_t e = cooperative ? cudaLaunchCooperativeKernel((void*)kernel, dim3(grid), dim3(block), argv, smem_bytes, W->stream)
+                                      : cudaLaunchKernel((void*)kernel, dim3(grid), dim3(block), argv, smem_bytes, W->stream);
+    const cudaError_t last = cudaGetLastError();
+    if (e != cudaSuccess || last != cudaSuccess) return e != cudaSuccess ? e : last;
+#else
+    (void)grid; (void)block; (void)cooperative;
+    const int floats = (int)(smem_bytes / 4);
+    if ((int)W->emu_smem.size() < floats) W->emu_smem.resize(floats);
+    emu_smem.p = W->emu_smem.data();
+    emu_smem.budget = std::min(floats, W->emu_coop_floats);
+    kernel(args...);
+#endif
+    W->kernels++;
+    return cudaSuccess;
+}
 
 template <class T>
 static int alloc_arr(RbWorld* W, T** p, size_t count) {
@@ -846,31 +882,18 @@ static int host_mass_props(const RbWorld* W, std::vector<HostMass>& out, int fir
 }
 
 static int launch_init_bodies(RbWorld* W, int first = 0) {
-#if RB_DEVICE_BUILD
-    int blocks = (W->w.nb - first + 255) / 256;
-    if (blocks < 1) blocks = 1;
-    k_init_bodies<<<blocks, 256, 0, W->stream>>>(W->w, first);
-    CK(cudaGetLastError());
-    W->kernels++;
-#else
-    GridCtx ctx;
-    init_bodies_phase(ctx, W->w, first);
-#endif
+    CK(launch(W, k_init_bodies, std::max((W->w.nb - first + 255) / 256, 1), 256, 0, false, W->w, first));
     return RB_OK;
 }
 
 // Waits for the world's stream.  `check`: also report (and clear) a status the device raised since the last check --
 // capacity overflow or non-finite state -- so asynchronous stepping (sync = 0, rb_world_step_host) cannot hide it.
 static int sync_world(RbWorld* W, bool check = true) {
-#if RB_DEVICE_BUILD
-    CK(cudaStreamSynchronize(W->stream));
+    CK(stream_sync(W->stream));
     if (W->host_hint && W->w.st && *(volatile int*)(W->host_hint + 3) != 0) {   // CCD clamps queued by the last step: apply them now
-        k_ccd_pending<<<1, 256, 0, W->stream>>>(W->w);
-        CK(cudaGetLastError());
-        W->kernels++;
-        CK(cudaStreamSynchronize(W->stream));
+        CK(launch(W, k_ccd_pending, 1, 256, 0, false, W->w));
+        CK(stream_sync(W->stream));
     }
-#endif
     if (check && W->host_hint && W->w.st) {
         const int code = *(volatile int*)(W->host_hint + 1);
         if (code != 0) {
@@ -1142,27 +1165,24 @@ RbWorld* rb_world_create(const RbIntegrationParameters* params, int device) {
     if (occ < 1) occ = 1;
     W->coop_blocks = W->num_sms * occ;
     W->coop_blocks_big = W->num_sms;
+#else
+    {   // emulated CTA: a test override of the shared-memory budget of both launch shapes that forces streaming
+        const char* v = getenv("RB_EMU_COOP_SMEM_FLOATS");
+        if (v) W->emu_coop_floats = atoi(v);
+        W->host_hint = W->emu_hint;
+    }
+#endif
     {   // debugging override (never needed in production): force the launch shape of k_solve_coop
         const char* v = getenv("RB_COOP_SHAPE");
         W->coop_shape = v ? atoi(v) : -1;
     }
-#else
-    {   // emulated CTA: shared-memory size of the big launch shape, or a test override that forces streaming
-        const char* v = getenv("RB_EMU_COOP_SMEM_FLOATS");
-        W->emu_coop_floats = v ? atoi(v) : COOP_BIG_SMEM_BYTES / 4;
-        W->emu_smem.assign(ITEM_MAX_BODIES * SB_STRIDE + W->emu_coop_floats, 0.0f);
-        W->host_hint = W->emu_hint;
-    }
-#endif
     return W;
 }
 
 void rb_world_destroy(RbWorld* W) {
     if (!W) return;
-#if RB_DEVICE_BUILD
-    cudaSetDevice(W->device);
-    cudaStreamSynchronize(W->stream);
-#endif
+    set_device(W->device);
+    stream_sync(W->stream);
     free_all(W);
 #if RB_DEVICE_BUILD
     for (cudaEvent_t e : W->prof_ev) cudaEventDestroy(e);
@@ -1294,10 +1314,8 @@ int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t
         set_err("invalid scene arguments%s", "");
         return RB_ERR_INVALID;
     }
-#if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
-    CK(cudaStreamSynchronize(W->stream));
-#endif
+    CK(set_device(W->device));
+    CK(stream_sync(W->stream));
     { int vrc = validate_descs(nb, nb, bodies, nc, colliders, (int)W->hulls.size()); if (vrc != RB_OK) return vrc; }
     for (int i = 0; i < nj; ++i) {
         const RbJointDesc& j = joints[i];
@@ -1671,19 +1689,11 @@ static int wake_impl(RbWorld* W, const int32_t* indices_host, int n) {
         if (dev_alloc((void**)&idx_dev, (size_t)std::max(n, 1) * sizeof(int)) != cudaSuccess) { set_err("device allocation failed%s", ""); return RB_ERR_CUDA; }
         CK(h2d(idx_dev, indices_host, (size_t)n * sizeof(int)));
     }
-#if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
+    CK(set_device(W->device));
     const int work = indices_host ? n : W->w.nb;
-    k_wake<<<(std::max(work, 1) + 255) / 256, 256, 0, W->stream>>>(W->w, idx_dev, n);
-    if (indices_host) k_wake_apply<<<(std::max(W->w.nb, 1) + 255) / 256, 256, 0, W->stream>>>(W->w);
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(W->stream));
-    W->kernels += 2;
-#else
-    GridCtx g;
-    wake_phase(g, W->w, idx_dev, n);
-    if (indices_host) wake_apply_phase(g, W->w);
-#endif
+    CK(launch(W, k_wake, (std::max(work, 1) + 255) / 256, 256, 0, false, W->w, idx_dev, n));
+    if (indices_host) CK(launch(W, k_wake_apply, (std::max(W->w.nb, 1) + 255) / 256, 256, 0, false, W->w));
+    CK(stream_sync(W->stream));
     if (idx_dev) dev_free(idx_dev);
     return RB_OK;
 }
@@ -1862,139 +1872,76 @@ int rb_world_step(RbWorld* W, const float gravity[3], int32_t nsteps, int32_t sy
     if (!W || !gravity || nsteps < 0) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
     if (W->w.nb == 0 && W->w.nc == 0) return RB_OK;
     Grav g{gravity[0], gravity[1], gravity[2]};
+    CK(set_device(W->device));
 #if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
     if (W->profiling) {
         while ((int)W->prof_ev.size() < 3 * nsteps) { cudaEvent_t e; CK(cudaEventCreate(&e)); W->prof_ev.push_back(e); }
         W->prof_steps = nsteps;
     }
+    // event i of step s: 0 before k_collide, 1 after it, 2 after the solves
+    auto mark = [&](int s, int i) { return W->profiling ? cudaEventRecord(W->prof_ev[3 * s + i], W->stream) : cudaSuccess; };
+#else
+    auto mark = [](int, int) { return cudaSuccess; };
+#endif
     for (int s = 0; s < nsteps; ++s) {
-        bool prof = W->profiling;
-        if (prof) CK(cudaEventRecord(W->prof_ev[3 * s], W->stream));
+        CK(mark(s, 0));
         // a grid-wide island existed after the last schedule the host knows of: it gets its own launch
         const bool general = general_path(W->w);
         const bool large = *(volatile int*)(W->host_hint + 2) != 0;
-        int do_solve = general ? 0 : (large ? 3 : 1);
+        const int do_solve = general ? 0 : (large ? 3 : 1);
         if (W->state_buf[1]) { W->w.state13 = W->state_buf[W->state_next]; W->state_next ^= 1; }
         // A new scene's islands are only known after its first schedule.  A caller that enqueues many steps in
         // one asynchronous call would otherwise run all of them in the launch shape chosen before that, so the
         // first call after a scene upload waits ONCE, after its second step, for the device hint.
-        if (W->steps_since_scene == 2 && nsteps > 3) CK(cudaStreamSynchronize(W->stream));
+        if (W->steps_since_scene == 2 && nsteps > 3) CK(stream_sync(W->stream));
         W->steps_since_scene++;
         // launch shape of k_solve_coop for this step (both kernels must agree on it): device hint of the last step
         const bool big = W->coop_shape >= 0 ? W->coop_shape == 1 : (*(volatile int*)W->host_hint != 0);
         W->w.step_index = (int)(W->steps + s + 1);
-        void* a1[] = {(void*)&W->w, (void*)&g, (void*)&do_solve};
-        CK(cudaLaunchCooperativeKernel(W->ext_shapes ? (void*)k_collide<1> : (void*)k_collide<0>, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a1, ITEM_SMEM_BYTES, W->stream));
-        if (prof) CK(cudaEventRecord(W->prof_ev[3 * s + 1], W->stream));
+        CK(launch(W, W->ext_shapes ? k_collide<1> : k_collide<0>, W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, true, W->w, g, do_solve));
+        CK(mark(s, 1));
         if (general) {   // every item through the streaming solve; the grid-wide item's kernel returns at once when there is none
-            void* a2[] = {(void*)&W->w, (void*)&g};
             // substep solve-groups: one pass of both kernels per distinct key, each with the parameters of its cadence
             const size_t npass = W->w.any_extra ? W->extra_keys.size() : 1;
             for (size_t ki = 0; ki < npass; ++ki) {
                 if (W->w.any_extra) {
                     W->w.pass_key = W->extra_keys[ki];
                     derive_params(W->params, W->w.prm, W->w.pass_key);
-                    if (ki > 0) CK(cudaMemsetAsync(&W->w.st->cursor_rest, 0, sizeof(int), W->stream));
+                    if (ki > 0) CK(memset_async(&W->w.st->cursor_rest, 0, sizeof(int), W->stream));
                 }
                 CK(with_variant(W->w, [&](auto fm, auto jm) {
                     constexpr int FM = decltype(fm)::value, JM = decltype(jm)::value;
-                    k_solve_items_x<FM, JM><<<W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, W->stream>>>(W->w, g);
-                    return cudaLaunchCooperativeKernel((void*)k_solve_large_x<FM, JM>, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a2, 0, W->stream);
+                    const cudaError_t e = launch(W, k_solve_items_x<FM, JM>, W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, false, W->w, g);
+                    return e != cudaSuccess ? e : launch(W, k_solve_large_x<FM, JM>, W->collide_blocks, COLLIDE_THREADS, 0, true, W->w, g);
                 }));
-                W->kernels += 2;
             }
             if (W->w.any_extra) { W->w.pass_key = 0; derive_params(W->params, W->w.prm); }
-            if (W->force_events) { k_force_events<<<W->collide_blocks, 256, 0, W->stream>>>(W->w); W->kernels++; }
-            if (prof) CK(cudaEventRecord(W->prof_ev[3 * s + 2], W->stream));
-            W->kernels += 1;
-            continue;
+        } else {
+            if (large) CK(launch(W, k_solve_large, W->collide_blocks, COLLIDE_THREADS, 0, true, W->w, g));
+            if (big) CK(launch(W, k_solve_coop_big, W->coop_blocks_big, COOP_BIG_THREADS, COOP_BIG_SMEM_BYTES, false, W->w, g));
+            else CK(launch(W, k_solve_coop, W->coop_blocks, COOP_SMALL_THREADS, COOP_SMALL_SMEM_BYTES, false, W->w, g));
         }
-        if (large) {
-            void* a2[] = {(void*)&W->w, (void*)&g};
-            CK(cudaLaunchCooperativeKernel((void*)k_solve_large, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a2, 0, W->stream));
-            W->kernels++;
-        }
-        if (big) k_solve_coop_big<<<W->coop_blocks_big, COOP_BIG_THREADS, COOP_BIG_SMEM_BYTES, W->stream>>>(W->w, g);
-        else k_solve_coop<<<W->coop_blocks, COOP_SMALL_THREADS, COOP_SMALL_SMEM_BYTES, W->stream>>>(W->w, g);
-        if (W->force_events) { k_force_events<<<W->collide_blocks, 256, 0, W->stream>>>(W->w); W->kernels++; }
-        CK(cudaGetLastError());
-        if (prof) CK(cudaEventRecord(W->prof_ev[3 * s + 2], W->stream));
-        W->kernels += 2;
+        if (W->force_events) CK(launch(W, k_force_events, W->collide_blocks, 256, 0, false, W->w));
+        CK(mark(s, 2));
     }
     W->steps += nsteps;
-    if (sync) {
-        CK(cudaStreamSynchronize(W->stream));
-        if (W->profiling && nsteps > 0) {  // mean per-step device time of each launch group over this call
-            float c = 0.f, v = 0.f;
-            for (int s = 0; s < W->prof_steps; ++s) {
-                float a = 0.f, b = 0.f;
-                cudaEventElapsedTime(&a, W->prof_ev[3 * s], W->prof_ev[3 * s + 1]);
-                cudaEventElapsedTime(&b, W->prof_ev[3 * s + 1], W->prof_ev[3 * s + 2]);
-                c += a; v += b;
-            }
-            W->ms_collide = c / W->prof_steps;
-            W->ms_solve = v / W->prof_steps;
-            W->ms_step = W->ms_collide + W->ms_solve;
+    if (!sync) return RB_OK;
+    CK(stream_sync(W->stream));
+#if RB_DEVICE_BUILD
+    if (W->profiling && nsteps > 0) {  // mean per-step device time of each launch group over this call
+        float c = 0.f, v = 0.f;
+        for (int s = 0; s < W->prof_steps; ++s) {
+            float a = 0.f, b = 0.f;
+            cudaEventElapsedTime(&a, W->prof_ev[3 * s], W->prof_ev[3 * s + 1]);
+            cudaEventElapsedTime(&b, W->prof_ev[3 * s + 1], W->prof_ev[3 * s + 2]);
+            c += a; v += b;
         }
-        return sync_world(W);
+        W->ms_collide = c / W->prof_steps;
+        W->ms_solve = v / W->prof_steps;
+        W->ms_step = W->ms_collide + W->ms_solve;
     }
-#else
-    for (int s = 0; s < nsteps; ++s) {
-        GridCtx gctx;
-        W->w.step_index = (int)(W->steps + s + 1);
-        if (W->state_buf[1]) { W->w.state13 = W->state_buf[W->state_next]; W->state_next ^= 1; }
-        W->emu_hint[0] = W->w.st->need_big;
-        W->w.st->need_big = W->w.st->coop_streamed = W->w.st->coop_resident = 0;
-        collide_pipeline<1>(gctx, W->w);   // (the emulation always carries the capsule code)
-        BlockCtx bctx;
-        SmemBodies sb;
-        sb.s = W->emu_smem.data();
-        BlockExec bex;
-        bex.c = &bctx;
-        int n = W->w.st->nitems;
-        CoopPipe pp;
-        unsigned long long mbar[2] = {0, 0};
-        pp.mbar = mbar;
-        pp.t = 0;
-        pp.sweep_threads = 1;
-        const size_t npass = W->w.any_extra ? W->extra_keys.size() : 1;   // substep solve-groups: one pass per distinct key
-        for (size_t ki = 0; ki < npass; ++ki) {
-        if (W->w.any_extra) { W->w.pass_key = W->extra_keys[ki]; derive_params(W->params, W->w.prm, W->w.pass_key); }
-        const bool general = general_path(W->w);
-        for (int k = 0; k < W->w.st->norder; ++k) {
-            const int item = W->w.item_order[k];
-            if (general)
-                with_variant(W->w, [&](auto fm, auto jm) { solve_item<HbmRows<decltype(fm)::value, decltype(jm)::value>>(bex, W->w, sb, item, mk3(g.x, g.y, g.z)); });
-            else if (item_is_coop(W->w, item))
-                solve_item_coop<1>(bctx, W->w, W->emu_smem.data() + ITEM_MAX_BODIES * SB_STRIDE, W->emu_coop_floats, pp, item, mk3(g.x, g.y, g.z));
-            else solve_item<HbmRows<0, 0>>(bex, W->w, sb, item, mk3(g.x, g.y, g.z));
-        }
-        if (W->w.st->nlarge_bodies > 0) {
-            GlobalBodies gb;
-            gb.w = &W->w;
-            GridExec gex;
-            gex.c = &gctx;
-            if (general)
-                with_variant(W->w, [&](auto fm, auto jm) { solve_item<HbmRows<decltype(fm)::value, decltype(jm)::value>>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z)); });
-            else solve_item<PoolRows<1>>(gex, W->w, gb, 0, mk3(g.x, g.y, g.z));
-        }
-        }
-        if (W->w.any_extra) { W->w.pass_key = 0; derive_params(W->params, W->w.prm); }
-        if (W->force_events) phase_force_events(gctx, W->w);
-        if (W->w.st->nccd > 0) {   // the queued CCD clamps (the device applies them at the next k_collide / synchronising call)
-            phase_ccd_pending(gctx, W->w, W->w.st->nccd, false);
-            if (W->w.st->nccd_bullets > 0) phase_ccd_pending(gctx, W->w, W->w.st->nccd, true);
-            W->w.st->nccd = 0;
-            W->w.st->nccd_bullets = 0;
-            W->w.host_hint[3] = 0;
-        }
-        W->kernels += 2;
-    }
-    W->steps += nsteps;
-    if (sync) return sync_world(W);
 #endif
-    return RB_OK;
+    return sync_world(W);
 }
 
 int rb_world_synchronize(RbWorld* W) {
@@ -2232,13 +2179,8 @@ int rb_debug_kat(const char* name, const float* in, int32_t n_in, float* out, in
         ALLOC(w.pb[0].rows, PR_ROWS); ALLOC(w.cons_hdr, 1); ALLOC(w.cons, CR_ROWS); ALLOC(w.item_flags, 2);
         ALLOC(din, n_in); ALLOC(dout, nout);
         CK(h2d(din, in, (size_t)n_in * sizeof(float)));
-#if RB_DEVICE_BUILD
-        k_kat<<<1, 1>>>(w, which, din, dout);
-        CK(cudaGetLastError());
-        CK(cudaDeviceSynchronize());
-#else
-        kat_phase(w, which, din, dout);
-#endif
+        CK(launch(W, k_kat, 1, 1, 0, false, w, which, din, dout));
+        CK(stream_sync(W->stream));
         CK(d2h(out, dout, (size_t)nout * sizeof(float)));
         return RB_OK;
     };
@@ -2251,21 +2193,11 @@ int rb_debug_kat(const char* name, const float* in, int32_t n_in, float* out, in
 int rb_world_label_components(RbWorld* W, int32_t* component_of_body) {
     if (!W || !component_of_body) return RB_ERR_INVALID;
     // Run the collision pipeline once (it leaves poses untouched) so the island labels are current.
-#if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
+    CK(set_device(W->device));
     int one = 1;
-    CK(cudaStreamSynchronize(W->stream));
+    CK(stream_sync(W->stream));
     CK(h2d(&W->w.st->sched_dirty, &one, sizeof(int)));
-    Grav g0{0.f, 0.f, 0.f};
-    int do_solve = 0;
-    void* a1[] = {(void*)&W->w, (void*)&g0, (void*)&do_solve};
-    CK(cudaLaunchCooperativeKernel(W->ext_shapes ? (void*)k_collide<1> : (void*)k_collide<0>, dim3(W->collide_blocks), dim3(COLLIDE_THREADS), a1, ITEM_SMEM_BYTES, W->stream));
-    W->kernels++;
-#else
-    W->w.st->sched_dirty = 1;
-    GridCtx g;
-    collide_pipeline<1>(g, W->w);
-#endif
+    CK(launch(W, W->ext_shapes ? k_collide<1> : k_collide<0>, W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, true, W->w, Grav{0.f, 0.f, 0.f}, 0));
     int rc = sync_world(W);
     if (rc != RB_OK) return rc;
     CK(d2h(component_of_body, W->w.isl_label, (size_t)W->w.nb * sizeof(int)));
@@ -2298,29 +2230,15 @@ int rb_world_set_owned_bodies(RbWorld* W, const uint8_t* owned) {
 // Stream-ordered, no host synchronisation; contact state of everything else is untouched.
 int rb_world_set_halo_bodies(RbWorld* W, const uint8_t* flags_dev) {
     if (!W || !flags_dev) return RB_ERR_INVALID;
-#if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
-    k_set_halo<<<(W->w.nb + 255) / 256, 256, 0, W->stream>>>(W->w, flags_dev);
-    CK(cudaGetLastError());
-    W->kernels++;
-#else
-    GridCtx g;
-    set_halo_phase(g, W->w, flags_dev);
-#endif
+    CK(set_device(W->device));
+    CK(launch(W, k_set_halo, (W->w.nb + 255) / 256, 256, 0, false, W->w, flags_dev));
     return RB_OK;
 }
 // Imports the states of the halo bodies from the packed state table (after an exchange wrote their rows).
 int rb_world_import_halo(RbWorld* W) {
     if (!W) return RB_ERR_INVALID;
-#if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
-    k_import_halo<<<(W->w.nb + 255) / 256, 256, 0, W->stream>>>(W->w);
-    CK(cudaGetLastError());
-    W->kernels++;
-#else
-    GridCtx g;
-    import_halo_phase(g, W->w);
-#endif
+    CK(set_device(W->device));
+    CK(launch(W, k_import_halo, (W->w.nb + 255) / 256, 256, 0, false, W->w));
     return RB_OK;
 }
 
@@ -2334,15 +2252,8 @@ int rb_world_state_buffer(RbWorld* W, void** device_ptr, int64_t* bytes) {
 static int import_states_impl(RbWorld* W, const int32_t* idx_dev, const float* src_dev, int32_t n, int table) {
     if (!W || n < 0) return RB_ERR_INVALID;
     if (n == 0) return RB_OK;
-#if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
-    k_import_states<<<(n + 255) / 256, 256, 0, W->stream>>>(W->w, idx_dev, src_dev, n, table);
-    CK(cudaGetLastError());
-    W->kernels++;
-#else
-    GridCtx g;
-    import_states_phase(g, W->w, idx_dev, src_dev, n, table);
-#endif
+    CK(set_device(W->device));
+    CK(launch(W, k_import_states, (n + 255) / 256, 256, 0, false, W->w, idx_dev, src_dev, n, table));
     return RB_OK;
 }
 // Imports externally simulated body states (device pointers): idx[n] body indices, src[n*13].
@@ -2365,13 +2276,9 @@ int rb_world_state_buffers(RbWorld* W, void** ptr0, void** ptr1, int64_t* bytes)
         if (rc != RB_OK) return rc;
         W->state_buf[0] = W->w.state13;
         W->state_buf[1] = second;
-#if RB_DEVICE_BUILD
-        CK(cudaSetDevice(W->device));
-        CK(cudaMemcpyAsync(second, W->w.state13, n * sizeof(float), cudaMemcpyDeviceToDevice, W->stream));
-        CK(cudaStreamSynchronize(W->stream));
-#else
-        memcpy(second, W->w.state13, n * sizeof(float));
-#endif
+        CK(set_device(W->device));
+        CK(copy_async(second, W->w.state13, n * sizeof(float), cudaMemcpyDeviceToDevice, W->stream));
+        CK(stream_sync(W->stream));
         W->state_next = 0;
     }
     *ptr0 = W->state_buf[0]; *ptr1 = W->state_buf[1];
@@ -2380,14 +2287,7 @@ int rb_world_state_buffers(RbWorld* W, void** ptr0, void** ptr1, int64_t* bytes)
 }
 
 // CUDA stream of the world (for callers that enqueue NCCL work behind the step).
-void* rb_world_stream(RbWorld* W) {
-#if RB_DEVICE_BUILD
-    return W ? (void*)W->stream : nullptr;
-#else
-    (void)W;
-    return nullptr;
-#endif
-}
+void* rb_world_stream(RbWorld* W) { return W ? (void*)W->stream : nullptr; }
 
 
 // Use a caller-provided CUDA stream (e.g. torch's current stream) for all of this world's work.
@@ -2410,54 +2310,40 @@ int rb_world_set_stream(RbWorld* W, void* stream) {
 int rb_world_step_host(RbWorld* W, const float gravity[3], const float* in_state13, float* out_state13) {
     if (!W || !gravity) return RB_ERR_INVALID;
     const size_t n = (size_t)W->w.nb * 13;
-#if RB_DEVICE_BUILD
-    CK(cudaSetDevice(W->device));
+    CK(set_device(W->device));
     // Page-locked caller buffers (cudaHostAlloc / cudaHostRegister / torch pin_memory) are DMA'd directly;
-    // pageable ones are staged through the library's pinned buffer.
+    // pageable ones are staged through the library's pinned buffer.  (The emulation stages every buffer.)
     auto is_pinned = [](const void* p) {
+#if RB_DEVICE_BUILD
         cudaPointerAttributes a;
         if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
         return a.type == cudaMemoryTypeHost;
-    };
+#else
+        (void)p;
+        return false;
 #endif
+    };
     if (in_state13) {
-#if RB_DEVICE_BUILD
         const float* src = in_state13;
         if (!is_pinned(in_state13)) { memcpy(W->stage_host, in_state13, n * sizeof(float)); src = W->stage_host; }
-        CK(cudaMemcpyAsync(W->stage_dev, src, n * sizeof(float), cudaMemcpyHostToDevice, W->stream));
-#else
-        memcpy(W->stage_dev, in_state13, n * sizeof(float));
-#endif
+        CK(copy_async(W->stage_dev, src, n * sizeof(float), cudaMemcpyHostToDevice, W->stream));
         int rc = rb_world_import_states(W, W->ident_dev, W->stage_dev, W->w.nb);
         if (rc != RB_OK) return rc;
     }
     int rc = rb_world_step(W, gravity, 1, 0);
     if (rc != RB_OK) return rc;
     if (out_state13) {
-#if RB_DEVICE_BUILD
-        if (is_pinned(out_state13)) {
-            CK(cudaMemcpyAsync(out_state13, W->w.state13, n * sizeof(float), cudaMemcpyDeviceToHost, W->stream));
-            CK(cudaStreamSynchronize(W->stream));
-            if (*(volatile int*)(W->host_hint + 3) != 0) {   // CCD clamps were queued by this step: apply them and fetch the state again
-                int rc2 = sync_world(W, false);
-                if (rc2 != RB_OK) return rc2;
-                CK(cudaMemcpyAsync(out_state13, W->w.state13, n * sizeof(float), cudaMemcpyDeviceToHost, W->stream));
-                CK(cudaStreamSynchronize(W->stream));
-            }
-        } else {
-            CK(cudaMemcpyAsync(W->stage_host + n, W->w.state13, n * sizeof(float), cudaMemcpyDeviceToHost, W->stream));
-            CK(cudaStreamSynchronize(W->stream));
-            if (*(volatile int*)(W->host_hint + 3) != 0) {
-                int rc2 = sync_world(W, false);
-                if (rc2 != RB_OK) return rc2;
-                CK(cudaMemcpyAsync(W->stage_host + n, W->w.state13, n * sizeof(float), cudaMemcpyDeviceToHost, W->stream));
-                CK(cudaStreamSynchronize(W->stream));
-            }
-            memcpy(out_state13, W->stage_host + n, n * sizeof(float));
+        float* dst = is_pinned(out_state13) ? out_state13 : W->stage_host + n;
+        auto fetch = [&]() {
+            const cudaError_t e = copy_async(dst, W->w.state13, n * sizeof(float), cudaMemcpyDeviceToHost, W->stream);
+            return e != cudaSuccess ? e : stream_sync(W->stream);
+        };
+        CK(fetch());
+        if (*(volatile int*)(W->host_hint + 3) != 0) {   // CCD clamps were queued by this step: apply them and fetch the state again
+            if ((rc = sync_world(W, false)) != RB_OK) return rc;
+            CK(fetch());
         }
-#else
-        memcpy(out_state13, W->w.state13, n * sizeof(float));
-#endif
+        if (dst != out_state13) memcpy(out_state13, dst, n * sizeof(float));
     }
     return sync_world(W);   // (the stream is idle by now: this only reports a status the device raised)
 }

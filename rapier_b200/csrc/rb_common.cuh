@@ -4,9 +4,15 @@
 // whose loops are strided by the context (grid-wide, CTA-wide or warp-wide) and whose phase
 // boundaries are ctx.grid_sync() / ctx.block_sync().  The product build (nvcc, sm_90a) instantiates
 // them with the CUDA contexts below inside __global__ kernels.  tests/emul/ compiles the very same
-// phase functions with g++ and a one-thread context (RB_EMULATE) so the kernel LOGIC can be checked
-// against the oracle on a machine without a GPU; that build is test infrastructure only and is never
-// loaded by the product (rapier_b200/_lib.py refuses to load anything but the CUDA library).
+// kernels and the host code that launches them with g++ and a one-thread context (RB_EMULATE): every
+// launch runs the kernel as one CTA of one thread, so the kernel logic and the host's step sequence can
+// be checked against the oracle on a machine without a GPU.  Kernels are spelled RB_KERNEL RB_BOUNDS(..),
+// take their dynamic shared memory through RB_DYNAMIC_SMEM and use RB_SHARED, ctx.block_sync() and
+// atomic_add instead of the CUDA spellings.  One thread has no lane groups, so the kernels that give a
+// constraint 4 lanes use 1 in the emulation (CONS_LANES, rb_api.cu), and the emulated shared-memory
+// budget of k_solve_coop can be lowered to force streaming (smem_budget).  That build is test
+// infrastructure only and is never loaded by the product (rapier_b200/_lib.py refuses to load
+// anything but the CUDA library).
 #pragma once
 #include <cstring>
 #include <stdint.h>
@@ -71,6 +77,11 @@ RB_D unsigned atomic_or(unsigned* p, unsigned v) { return atomicOr(p, v); }
 RB_D int atomic_cas(int* p, int cmp, int v) { return atomicCAS(p, cmp, v); }
 RB_D void thread_fence() { __threadfence(); }
 #define RB_SHARED __shared__
+#define RB_KERNEL __global__ void
+#define RB_BOUNDS(...) __launch_bounds__(__VA_ARGS__)
+#define RB_DYNAMIC_SMEM(name) extern __shared__ __align__(16) float name[]
+// Shared-memory budget (floats) a kernel plans with, given the dynamic shared memory it is launched with.
+RB_D int smem_budget(int floats) { return floats; }
 
 #else  // ---------------- host emulation: one thread plays every role ----------------
 
@@ -93,6 +104,14 @@ inline unsigned atomic_or(unsigned* p, unsigned v) { unsigned o = *p; *p = o | v
 inline int atomic_cas(int* p, int cmp, int v) { int o = *p; if (o == cmp) *p = v; return o; }
 inline void thread_fence() {}
 #define RB_SHARED static
+#define RB_KERNEL inline void
+#define RB_BOUNDS(...)
+// The launcher (rb_api.cu launch()) provides the dynamic shared memory of each emulated kernel, and the budget it
+// may plan with: at most what it was launched with, lowered by RB_EMU_COOP_SMEM_FLOATS.
+struct EmuSmem { float* p = nullptr; int budget = 0; };
+inline EmuSmem emu_smem;
+#define RB_DYNAMIC_SMEM(name) float* const name = ::rb::emu_smem.p
+inline int smem_budget(int floats) { return floats < emu_smem.budget ? floats : emu_smem.budget; }
 
 #endif
 
