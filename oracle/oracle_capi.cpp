@@ -310,6 +310,22 @@ int64_t orc_world_debug_read(OrcWorld* o, const char* table, void* dst, int64_t 
             put<float>(b, q.eff_world_inv_inertia.m13); put<float>(b, q.eff_world_inv_inertia.m22);
             put<float>(b, q.eff_world_inv_inertia.m23); put<float>(b, q.eff_world_inv_inertia.m33);
         }
+    } else if (t == "body_mframe") {  // principal frame xyzw, effective inverse mass xyz
+        for (const Body& q : w.bodies) {
+            put<float>(b, q.principal_frame.x); put<float>(b, q.principal_frame.y); put<float>(b, q.principal_frame.z);
+            put<float>(b, q.principal_frame.w); put3(b, q.eff_inv_mass);
+        }
+    } else if (t == "hull_tables") {  // the layout of rb_world_debug_read's table, over every registered hull
+        for (const Hull& h : w.hulls) {
+            const int nv = (int)h.verts.size(), nf = (int)h.face_count.size(), ne = (int)h.edges.size(), nl = (int)h.loops.size();
+            put<int32_t>(b, nv); put<int32_t>(b, nf); put<int32_t>(b, ne); put<int32_t>(b, nl);
+            put3(b, h.aabb); put<float>(b, h.radius);
+            for (const V3& v : h.verts) put3(b, v);
+            for (int f = 0; f < nf; ++f) { put3(b, h.normals[f]); put<float>(b, h.offsets[f]); }
+            for (int f = 0; f < nf; ++f) { put<int32_t>(b, h.face_start[f]); put<int32_t>(b, h.face_count[f]); }
+            for (int l : h.loops) put<int32_t>(b, l);
+            for (const HullEdge& e : h.edges) { put<int32_t>(b, e.v0); put<int32_t>(b, e.v1); put<int32_t>(b, e.f0); put<int32_t>(b, e.f1); }
+        }
     } else if (t == "joint_impulses") {
         for (const Joint& j : w.joints)
             for (int k = 0; k < 6; ++k) put<float>(b, j.impulses[k]);

@@ -206,7 +206,7 @@ static int recompute_mass_properties(World& w, int first_body = 0, int first_col
                 M = M + mass;
                 com = com + c.pos_wrt_parent.t * mass;
             }
-            if (M == 0.0f) continue;
+            if (M != 0.0f) {   // (a massless compound still reaches the additional mass and the extents below)
             com = com * (1.0f / M);
             bool simple = true;   // axis-aligned parts offset from the centre of mass along one axis: the summed tensor is diagonal
             for (size_t ci = (size_t)first_collider; ci < w.colliders.size(); ++ci) {
@@ -252,6 +252,7 @@ static int recompute_mass_properties(World& w, int first_body = 0, int first_col
                 b.inv_principal_inertia = V3{inv_exact0(I[0]), inv_exact0(I[1]), inv_exact0(I[2])};
             }
             b.inv_mass = inv_exact0(M);
+            }
         }
         // RigidBodyAdditionalMassProps::Mass (rigid_body_components.rs:454-486); MassProperties::set_mass(m, true)
         // [parry] rescales the angular inertia by new_mass / old_mass, i.e. its inverse by inv(new) * old.

@@ -2130,6 +2130,38 @@ int64_t rb_world_debug_read(RbWorld* W, const char* table, void* dst, int64_t ca
         CK(d2h(wc.data(), W->w.b_wcom, (size_t)nb * 16)); CK(d2h(e0.data(), W->w.b_eii0, (size_t)nb * 16));
         CK(d2h(e1.data(), W->w.b_eii1, (size_t)nb * 8));
         for (int i = 0; i < nb; ++i) { put(&lc[i], 16); put(&ipi[i], 12); put(&wc[i], 12); put(&e0[i], 16); put(&e1[i], 8); }
+    } else if (t == "body_mframe") {   // principal frame xyzw, effective inverse mass xyz
+        int nb = W->w.nb;
+        std::vector<float4> fr(std::max(nb, 1)), eim(std::max(nb, 1));
+        CK(d2h(fr.data(), W->w.b_pframe, (size_t)nb * 16)); CK(d2h(eim.data(), W->w.b_eim, (size_t)nb * 16));
+        for (int i = 0; i < nb; ++i) { put(&fr[i], 16); put(&eim[i], 12); }
+    } else if (t == "hull_tables") {
+        // the device's polyhedron tables, hull by hull (none before a convex collider is uploaded), in 4-byte words:
+        // nv, nf, ne, nloop | aabb xyz, radius | verts [nv][3] | planes [nf][4] | faces [nf] (start, count) | loops [nloop] | edges [ne][4]
+        const int nh = W->w.hulls.desc ? W->hulls_uploaded : 0;
+        size_t tv = 0, tf = 0, te = 0, tl = 0;
+        for (int h = 0; h < nh; ++h) { tv += W->hulls[h].nv(); tf += W->hulls[h].nf(); te += W->hulls[h].ne(); tl += W->hulls[h].loops.size(); }
+        std::vector<int4> desc(std::max(nh, 1)), desc2(std::max(nh, 1)), edges(std::max(te, (size_t)1));
+        std::vector<float4> info(std::max(nh, 1)), verts(std::max(tv, (size_t)1)), planes(std::max(tf, (size_t)1));
+        std::vector<int2> faces(std::max(tf, (size_t)1));
+        std::vector<int> loops(std::max(tl, (size_t)1));
+        if (nh) {
+            CK(d2h(desc.data(), W->w.hulls.desc, nh * sizeof(int4))); CK(d2h(desc2.data(), W->w.hulls.desc2, nh * sizeof(int4)));
+            CK(d2h(info.data(), W->w.hulls.info, nh * sizeof(float4))); CK(d2h(verts.data(), W->w.hulls.verts, tv * sizeof(float4)));
+            CK(d2h(planes.data(), W->w.hulls.planes, tf * sizeof(float4))); CK(d2h(faces.data(), W->w.hulls.faces, tf * sizeof(int2)));
+            CK(d2h(loops.data(), W->w.hulls.loops, tl * sizeof(int))); CK(d2h(edges.data(), W->w.hulls.edges, te * sizeof(int4)));
+        }
+        for (int h = 0; h < nh; ++h) {
+            const int4 d = desc[h], d2 = desc2[h];
+            const int nloop = (h + 1 < nh ? desc2[h + 1].z : (int)tl) - d2.z;
+            const int hdr[4] = {d.y, d.w, d2.y, nloop};
+            put(hdr, 16); put(&info[h], 16);
+            for (int i = 0; i < d.y; ++i) put(&verts[d.x + i], 12);
+            for (int f = 0; f < d.w; ++f) put(&planes[d.z + f], 16);
+            for (int f = 0; f < d.w; ++f) put(&faces[d.z + f], 8);
+            put(loops.data() + d2.z, (size_t)nloop * 4);
+            for (int e = 0; e < d2.y; ++e) put(&edges[d2.x + e], 16);
+        }
     } else if (t == "joint_impulses") {
         std::vector<float> v((size_t)std::max(W->w.nj, 1) * 6);
         CK(d2h(v.data(), W->w.j_impulses, (size_t)W->w.nj * 24));

@@ -17,6 +17,7 @@
 namespace rbhull {
 
 constexpr int MAX_VERTS = 32, MAX_FACES = 32, MAX_FACE_VERTS = 8, MAX_EDGES = 64;
+constexpr double REPEAT_EPS = 4.0;   // convex_hull: repeat radius of the input points, in units of its plane tolerance
 
 struct Hull {
     std::vector<float> verts;                 // 3 * nv
@@ -215,11 +216,22 @@ inline const char* convex_hull(int np, const float* pts, std::vector<float>& out
     for (int i = 0; i < 3 * np; ++i) { if (!std::isfinite(pts[i])) return "non-finite point"; size = std::max(size, (double)std::fabs(pts[i])); }
     const double eps = 1.0e-6 * (1.0 + size);
     auto P = [&](int i, double o[3]) { for (int k = 0; k < 3; ++k) o[k] = pts[3 * i + k]; };
+    // A repeated point -- within REPEAT_EPS * eps of an earlier kept one in every coordinate -- takes no part (the earlier
+    // one stands for it).  Two such copies of one corner are both on or near every plane through it, and the faces around
+    // that corner would not all keep the same copy, leaving the mesh open; up to a few eps apart the tolerances of the plane
+    // membership and of the polygon turns still disagree about them.
+    const double rep = REPEAT_EPS * eps;
+    std::vector<char> dup(np, 0);
+    for (int i = 0; i < np; ++i)
+        for (int j = 0; j < i && !dup[i]; ++j)
+            dup[i] = !dup[j] && std::fabs((double)pts[3 * i] - pts[3 * j]) <= rep && std::fabs((double)pts[3 * i + 1] - pts[3 * j + 1]) <= rep &&
+                     std::fabs((double)pts[3 * i + 2] - pts[3 * j + 2]) <= rep;
     std::vector<uint32_t> seen;            // vertex masks of the faces found
     std::vector<std::vector<int>> faces;
     for (int i = 0; i < np; ++i)
         for (int j = i + 1; j < np; ++j)
             for (int k = j + 1; k < np; ++k) {
+                if (dup[i] || dup[j] || dup[k]) continue;
                 double a[3], b[3], c[3], ab[3], ac[3], n[3];
                 P(i, a); P(j, b); P(k, c);
                 for (int t = 0; t < 3; ++t) { ab[t] = b[t] - a[t]; ac[t] = c[t] - a[t]; }
@@ -231,6 +243,7 @@ inline const char* convex_hull(int np, const float* pts, std::vector<float>& out
                 int pos = 0, neg = 0;
                 uint32_t mask = 0;
                 for (int m = 0; m < np; ++m) {
+                    if (dup[m]) continue;
                     double q[3];
                     P(m, q);
                     const double s = dot3d(n, q) - d;
