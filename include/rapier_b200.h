@@ -11,6 +11,10 @@
  * entry points below with `extern "C"` (see INTEGRATION.md).  All pointers are caller-owned host
  * memory; the library copies.  One RbWorld is not re-entrant (the reference takes `&mut self`).
  * Every function returns RB_OK (0) or a negative RbStatus; rb_last_error() describes the failure.
+ * The calls that edit the sets -- rb_world_set_body_states, rb_world_set_body_forces, rb_world_set_next_kinematic_positions,
+ * rb_world_wake_up, rb_world_insert, rb_world_remove_bodies, rb_world_insert_joints, rb_world_remove_joints and
+ * rb_world_update_joints -- check all of their input before they change anything: a call that returns RB_ERR_INVALID
+ * has applied none of its entries and woken no body.
  * There is NO CPU fallback: without a CUDA device rb_world_create fails with RB_ERR_NO_DEVICE.
  */
 #ifndef RAPIER_B200_H

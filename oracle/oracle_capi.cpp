@@ -91,12 +91,17 @@ int orc_world_set_scene(OrcWorld* w, int32_t nb, const RbBodyDesc* bodies, int32
     if (!w) return RB_ERR_INVALID;
     return set_scene(w->w, nb, bodies, nc, colliders, nj, joints);
 }
+// rb_world_* checks every index of a set-editing call before it changes anything; so do these mirrors.
+static bool bodies_valid(const World& w, int n, const int32_t* indices, int type = -1) {
+    for (int k = 0; k < n; ++k)
+        if (indices[k] < 0 || indices[k] >= (int)w.bodies.size() || (type >= 0 && w.bodies[indices[k]].type != type)) return false;
+    return true;
+}
 int orc_world_wake_up(OrcWorld* o, int32_t n, const int32_t* indices) {
-    if (!o || n < 0) return RB_ERR_INVALID;
+    if (!o || n < 0 || !bodies_valid(o->w, n, indices)) return RB_ERR_INVALID;
     World& w = o->w;
     for (int k = 0; k < n; ++k) {
         const int i = indices[k];
-        if (i < 0 || i >= (int)w.bodies.size()) return RB_ERR_INVALID;
         if (!w.bodies[i].is_dynamic()) continue;
         const int root = i < (int)w.island_of.size() ? w.island_of[i] : -1;
         for (int b = 0; b < (int)w.bodies.size(); ++b) {
@@ -143,11 +148,10 @@ int orc_world_remove_joints(OrcWorld* w, int32_t n, const int32_t* indices) {
     return remove_joints(w->w, n, indices);
 }
 int orc_world_set_body_states(OrcWorld* o, int32_t n, const int32_t* indices, const float* pose7, const float* vel6) {
-    if (!o) return RB_ERR_INVALID;
+    if (!o || n < 0 || !bodies_valid(o->w, n, indices)) return RB_ERR_INVALID;
     World& w = o->w;
     for (int k = 0; k < n; ++k) {
         int i = indices[k];
-        if (i < 0 || i >= (int)w.bodies.size()) return RB_ERR_INVALID;
         Body& b = w.bodies[i];
         if (pose7) {
             b.pos.t = V3{pose7[k * 7 + 0], pose7[k * 7 + 1], pose7[k * 7 + 2]};
@@ -167,22 +171,20 @@ int orc_world_set_body_states(OrcWorld* o, int32_t n, const int32_t* indices, co
     return orc_world_wake_up(o, n, indices);   // a user change wakes the body's island (user_changes.rs)
 }
 int orc_world_set_body_forces(OrcWorld* o, int32_t n, const int32_t* indices, const float* force3, const float* torque3) {
-    if (!o) return RB_ERR_INVALID;
+    if (!o || n < 0 || !bodies_valid(o->w, n, indices)) return RB_ERR_INVALID;
     World& w = o->w;
     for (int k = 0; k < n; ++k) {
         int i = indices[k];
-        if (i < 0 || i >= (int)w.bodies.size()) return RB_ERR_INVALID;
         if (force3) w.bodies[i].user_force = V3{force3[k * 3], force3[k * 3 + 1], force3[k * 3 + 2]};
         if (torque3) w.bodies[i].user_torque = V3{torque3[k * 3], torque3[k * 3 + 1], torque3[k * 3 + 2]};
     }
     return orc_world_wake_up(o, n, indices);
 }
 int orc_world_set_next_kinematic_positions(OrcWorld* o, int32_t n, const int32_t* indices, const float* pose7) {
-    if (!o || !pose7) return RB_ERR_INVALID;
+    if (!o || !pose7 || n < 0 || !bodies_valid(o->w, n, indices, RB_BODY_KINEMATIC_POSITION_BASED)) return RB_ERR_INVALID;
     World& w = o->w;
     for (int k = 0; k < n; ++k) {
         int i = indices[k];
-        if (i < 0 || i >= (int)w.bodies.size() || w.bodies[i].type != RB_BODY_KINEMATIC_POSITION_BASED) return RB_ERR_INVALID;
         w.bodies[i].kin_target = Pose{Q4{pose7[k * 7 + 3], pose7[k * 7 + 4], pose7[k * 7 + 5], pose7[k * 7 + 6]}, V3{pose7[k * 7], pose7[k * 7 + 1], pose7[k * 7 + 2]}};
     }
     return orc_world_wake_up(o, n, indices);

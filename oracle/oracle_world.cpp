@@ -1028,10 +1028,12 @@ int insert_joints(World& w, int n, const RbJointDesc* jd) {
 }
 static void wake_island_of(World& w, int body);
 int update_joints(World& w, int n, const int* indices, const RbJointDesc* jd, int wake_up) {   // rb_world_update_joints
-    for (int k = 0; k < n; ++k) {
+    for (int k = 0; k < n; ++k) {   // every entry is checked before any is applied
         if (indices[k] < 0 || indices[k] >= (int)w.joints.size() || w.joints[indices[k]].removed) return RB_ERR_INVALID;
+        if (jd[k].body1 != w.joints[indices[k]].body1 || jd[k].body2 != w.joints[indices[k]].body2) return RB_ERR_INVALID;
+    }
+    for (int k = 0; k < n; ++k) {
         Joint& j = w.joints[indices[k]];
-        if (jd[k].body1 != j.body1 || jd[k].body2 != j.body2) return RB_ERR_INVALID;
         float imp[3][6];
         for (int a = 0; a < 6; ++a) { imp[0][a] = j.impulses[a]; imp[1][a] = j.limit_impulses[a]; imp[2][a] = j.motor_impulses[a]; }
         int rc = fill_joint(w, j, jd[k]);
@@ -1044,10 +1046,9 @@ int update_joints(World& w, int n, const int* indices, const RbJointDesc* jd, in
     return RB_OK;
 }
 int remove_joints(World& w, int n, const int* indices) {
-    for (int k = 0; k < n; ++k) {
+    for (int k = 0; k < n; ++k)
         if (indices[k] < 0 || indices[k] >= (int)w.joints.size()) return RB_ERR_INVALID;
-        w.joints[indices[k]].removed = true;
-    }
+    for (int k = 0; k < n; ++k) w.joints[indices[k]].removed = true;
     refresh_joint_set(w);
     return RB_OK;
 }

@@ -14,6 +14,7 @@
 // step's launch sequence for machines without a GPU, never part of the product library.  It differs from
 // the device in two places: the 4-lane kernels run 1 lane per constraint (CONS_LANES), and
 // RB_EMU_COOP_SMEM_FLOATS can lower the shared-memory budget of both k_solve_coop launch shapes.
+#include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -33,7 +34,10 @@ using namespace rb;
 // error handling + memory backend
 // ------------------------------------------------------------------------------------------------
 static thread_local char g_err[512] = "";
-static void set_err(const char* fmt, const char* a = "", int code = 0) { snprintf(g_err, sizeof(g_err), fmt, a, code); }
+__attribute__((format(printf, 1, 2))) static void set_err(const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt); vsnprintf(g_err, sizeof(g_err), fmt, ap); va_end(ap);
+}
 
 #if RB_DEVICE_BUILD
 #define CK(call)                                                                 \
@@ -56,7 +60,7 @@ static cudaError_t copy_async(void* d, const void* h, size_t n, cudaMemcpyKind k
 #else
 #define CK(call)                                 \
     do {                                         \
-        if ((call) != 0) { set_err("emulated allocation failed%s", ""); return RB_ERR_CUDA; } \
+        if ((call) != 0) { set_err("emulated allocation failed"); return RB_ERR_CUDA; } \
     } while (0)
 static cudaError_t dev_alloc(void** p, size_t n) { *p = calloc(n ? n : 16, 1); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 static cudaError_t dev_free(void* p) { free(p); return cudaSuccess; }
@@ -489,6 +493,7 @@ struct RbWorld {
     int njused = 0;
     float* stage_dev = nullptr;      // [nb*13] device staging for bulk state import
     int* ident_dev = nullptr;        // [nb] identity index list
+    int* wake_idx = nullptr; int wake_cap = 0;   // [wake_cap] device copy of the body indices of the last wake_impl call
     float* stage_host = nullptr;     // pinned host staging (2 * nb * 13 floats: in, out)
     cudaStream_t stream = nullptr;   // (the emulation has none)
 #if RB_DEVICE_BUILD
@@ -528,7 +533,7 @@ static cudaError_t launch(RbWorld* W, void (*kernel)(P...), int grid, int block,
 template <class T>
 static int alloc_arr(RbWorld* W, T** p, size_t count) {
     void* v = nullptr;
-    if (dev_alloc(&v, count * sizeof(T)) != cudaSuccess) { set_err("device allocation failed%s", ""); return RB_ERR_CUDA; }
+    if (dev_alloc(&v, count * sizeof(T)) != cudaSuccess) { set_err("device allocation failed"); return RB_ERR_CUDA; }
     W->allocs.push_back(v);
     *p = (T*)v;
     return RB_OK;
@@ -617,11 +622,11 @@ static void refresh_extra_keys(RbWorld* W) {
 }
 
 static int validate_params(const RbIntegrationParameters* p) {
-    if (!p) { set_err("null parameters%s", ""); return RB_ERR_INVALID; }
-    if (p->friction_model != 0 && p->friction_model != 1) { set_err("friction_model must be 0 (Simplified) or 1 (Coulomb)%s", ""); return RB_ERR_INVALID; }
-    if (p->warmstart_joints != 0 && p->warmstart_joints != 1) { set_err("warmstart_joints must be 0 or 1%s", ""); return RB_ERR_INVALID; }
-    if (p->max_ccd_substeps < 0 || p->max_ccd_substeps > 1) { set_err("max_ccd_substeps must be 0 (CCD off) or 1 (motion clamping); the multi-substep splitter is not supported%s", ""); return RB_ERR_INVALID; }
-    if (p->num_solver_iterations < 1 || p->num_solver_iterations > 64) { set_err("num_solver_iterations out of range%s", ""); return RB_ERR_INVALID; }
+    if (!p) { set_err("null parameters"); return RB_ERR_INVALID; }
+    if (p->friction_model != 0 && p->friction_model != 1) { set_err("friction_model must be 0 (Simplified) or 1 (Coulomb)"); return RB_ERR_INVALID; }
+    if (p->warmstart_joints != 0 && p->warmstart_joints != 1) { set_err("warmstart_joints must be 0 or 1"); return RB_ERR_INVALID; }
+    if (p->max_ccd_substeps < 0 || p->max_ccd_substeps > 1) { set_err("max_ccd_substeps must be 0 (CCD off) or 1 (motion clamping); the multi-substep splitter is not supported"); return RB_ERR_INVALID; }
+    if (p->num_solver_iterations < 1 || p->num_solver_iterations > 64) { set_err("num_solver_iterations out of range"); return RB_ERR_INVALID; }
     return RB_OK;
 }
 
@@ -797,7 +802,7 @@ static int host_mass_props(const RbWorld* W, std::vector<HostMass>& out, int fir
             for (size_t ci = (size_t)first_collider; ci < W->colliders.size(); ++ci) {
                 const RbColliderDesc& c = W->colliders[ci];
                 if (c.parent != b || (c.sensor && c.density == 0.0f)) continue;
-                if (c.shape == RB_SHAPE_CONVEX) { set_err("multi-collider bodies with convex polyhedra are not supported%s", ""); return RB_ERR_INVALID; }
+                if (c.shape == RB_SHAPE_CONVEX) { set_err("multi-collider bodies with convex polyhedra are not supported"); return RB_ERR_INVALID; }
                 float mass, pi[3];
                 collider_mass_props(c, mass, pi);
                 M = M + mass;
@@ -859,7 +864,7 @@ static int host_mass_props(const RbWorld* W, std::vector<HostMass>& out, int fir
                 for (int k = 0; k < 3; ++k) m.ipi[k] = m.ipi[k] * (inv_new * prev);
                 m.inv_mass = inv_new;
             } else if (count[b] == 1 && W->colliders[first[b]].shape == RB_SHAPE_CONVEX) {
-                set_err("additional mass on a massless convex polyhedron is not supported%s", "");
+                set_err("additional mass on a massless convex polyhedron is not supported");
                 return RB_ERR_INVALID;
             } else if (count[b] == 1) {
                 // massless collider: inertia and centre of mass of the shape at unit density, rescaled to the mass
@@ -874,7 +879,7 @@ static int host_mass_props(const RbWorld* W, std::vector<HostMass>& out, int fir
             } else if (count[b] == 0) {
                 m.inv_mass = inv0(add);   // no shape to derive an inertia from: just the mass
             } else {
-                set_err("additional mass on a massless multi-collider body is not supported%s", "");
+                set_err("additional mass on a massless multi-collider body is not supported");
                 return RB_ERR_INVALID;
             }
         }
@@ -916,15 +921,46 @@ static int sync_world(RbWorld* W, bool check = true) {
             W->host_hint[1] = 0;
             int zero = 0;
             CK(h2d(&W->w.st->error, &zero, sizeof(int)));
-            set_err(code == -6 ? "device raised status %s%d (a contact formed between bodies simulated by different ranks: the shards' islands merged, repartition)" : code == RB_ERR_NONFINITE ? "device raised status %s%d (non-finite body state: see rb_world_get_quarantine)"
-                                             : "device raised status %s%d (capacity overflow: the step kept the previous pair set / truncated the schedule)", "", code);
+            set_err(code == -6 ? "device raised status %d (a contact formed between bodies simulated by different ranks: the shards' islands merged, repartition)" : code == RB_ERR_NONFINITE ? "device raised status %d (non-finite body state: see rb_world_get_quarantine)"
+                                             : "device raised status %d (capacity overflow: the step kept the previous pair set / truncated the schedule)", code);
             return code;
         }
     }
     return RB_OK;
 }
 
-extern "C" { static int wake_impl(RbWorld* W, const int32_t* indices_host, int n); }
+// Wakes the islands of the listed bodies (indices_host == NULL: every sleeping body) and waits for it.
+static int wake_impl(RbWorld* W, const int32_t* indices_host, int n) {
+    if (indices_host && n > W->wake_cap) {   // (the scratch only grows; the old one is freed with the world's tables)
+        const int cap = std::max(n, 2 * W->wake_cap);
+        ALLOC(W->wake_idx, cap);
+        W->wake_cap = cap;
+    }
+    if (indices_host) CK(h2d(W->wake_idx, indices_host, (size_t)n * sizeof(int)));
+    CK(set_device(W->device));
+    const int work = indices_host ? n : W->w.nb;
+    CK(launch(W, k_wake, (std::max(work, 1) + 255) / 256, 256, 0, false, W->w, indices_host ? W->wake_idx : nullptr, n));
+    if (indices_host) CK(launch(W, k_wake_apply, (std::max(W->w.nb, 1) + 255) / 256, 256, 0, false, W->w));
+    CK(stream_sync(W->stream));
+    return RB_OK;
+}
+
+// Checks every index of a set-editing call before it changes anything: each in [0, nb) and, for `type` >= 0, a body of
+// that type.  A rejected call has applied none of its entries.
+static int check_bodies(const RbWorld* W, int n, const int32_t* indices, const char* why = "body index out of range", int type = -1) {
+    for (int k = 0; k < n; ++k)
+        if (indices[k] < 0 || indices[k] >= W->w.nb || (type >= 0 && W->bodies[indices[k]].body_type != type)) { set_err("%s", why); return RB_ERR_INVALID; }
+    return RB_OK;
+}
+
+// Flags what the next step rebuilds: the broad-phase lists (1: movers, 3: static colliders too), the pair set, the islands and
+// the schedule.  A zero argument leaves that flag as it is.
+static int mark_dirty(RbWorld* W, int lists, int bp, int sched) {
+    if (lists) CK(h2d(&W->w.st->lists_dirty, &lists, sizeof(int)));
+    if (bp) CK(h2d(&W->w.st->bp_dirty, &bp, sizeof(int)));
+    if (sched) CK(h2d(&W->w.st->sched_dirty, &sched, sizeof(int)));
+    return RB_OK;
+}
 
 static int read_state(RbWorld* W, State& s) {
     int rc = sync_world(W, false);   // (counters / debug reads must stay readable after an overflow; they do not consume the status)
@@ -1095,13 +1131,13 @@ static int validate_descs(int nb_total, int nb, const RbBodyDesc* bodies, int nc
         const bool convex_ok = c.shape == RB_SHAPE_CONVEX && c.half_extents[0] >= 0.0f && c.half_extents[0] < (float)nhulls &&
                                c.half_extents[0] == (float)(int)c.half_extents[0] && c.half_extents[1] >= 0.0f;
         if ((c.shape != RB_SHAPE_BALL && c.shape != RB_SHAPE_CUBOID && !capsule_ok && !convex_ok) || c.parent >= nb_total) {
-            set_err("collider with unsupported shape, unknown hull or bad parent%s", "");
+            set_err("collider with unsupported shape, unknown hull or bad parent");
             return RB_ERR_INVALID;
         }
     }
     for (int i = 0; i < nb; ++i)
         if (bodies[i].body_type < RB_BODY_DYNAMIC || bodies[i].body_type > RB_BODY_KINEMATIC_VELOCITY_BASED) {
-            set_err("unknown body type%s", "");
+            set_err("unknown body type");
             return RB_ERR_INVALID;
         }
     return RB_OK;
@@ -1150,7 +1186,7 @@ RbWorld* rb_world_create(const RbIntegrationParameters* params, int device) {
                 e == cudaSuccess ? "device ordinal out of range" : cudaGetErrorString(e), (int)e);
         return nullptr;
     }
-    if (cudaSetDevice(device) != cudaSuccess) { set_err("cudaSetDevice failed%s", ""); return nullptr; }
+    if (cudaSetDevice(device) != cudaSuccess) { set_err("cudaSetDevice failed"); return nullptr; }
 #endif
     RbWorld* W = new RbWorld();
     W->params = *params;
@@ -1161,11 +1197,11 @@ RbWorld* rb_world_create(const RbIntegrationParameters* params, int device) {
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
     W->num_sms = prop.multiProcessorCount;
-    if (!prop.cooperativeLaunch) { set_err("device lacks cooperative launch%s", ""); delete W; return nullptr; }
+    if (!prop.cooperativeLaunch) { set_err("device lacks cooperative launch"); delete W; return nullptr; }
     cudaStreamCreateWithFlags(&W->stream, cudaStreamNonBlocking);
     cudaFuncSetAttribute(k_solve_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, COOP_SMALL_SMEM_BYTES);
     cudaFuncSetAttribute(k_solve_coop_big, cudaFuncAttributeMaxDynamicSharedMemorySize, COOP_BIG_SMEM_BYTES);
-    if (cudaHostAlloc((void**)&W->host_hint, 4 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) { set_err("cudaHostAlloc failed%s", ""); delete W; return nullptr; }
+    if (cudaHostAlloc((void**)&W->host_hint, 4 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) { set_err("cudaHostAlloc failed"); delete W; return nullptr; }
     for (int i = 0; i < 4; ++i) W->host_hint[i] = 0;
     cudaFuncSetAttribute(k_collide<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
     cudaFuncSetAttribute(k_collide<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ITEM_SMEM_BYTES);
@@ -1175,7 +1211,7 @@ RbWorld* rb_world_create(const RbIntegrationParameters* params, int device) {
         });
     int occ = 1;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_collide<1>, COLLIDE_THREADS, ITEM_SMEM_BYTES);
-    if (occ < 1) { set_err("k_collide cannot be resident%s", ""); delete W; return nullptr; }
+    if (occ < 1) { set_err("k_collide cannot be resident"); delete W; return nullptr; }
     W->collide_blocks = W->num_sms;   // one CTA per SM: the cheapest grid barrier that still covers the chip
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_solve_coop, COOP_SMALL_THREADS, COOP_SMALL_SMEM_BYTES);
     if (occ < 1) occ = 1;
@@ -1212,12 +1248,12 @@ void rb_world_destroy(RbWorld* W) {
 }
 
 int rb_world_set_params(RbWorld* W, const RbIntegrationParameters* params) {
-    if (!W) { set_err("null world%s", ""); return RB_ERR_INVALID; }
+    if (!W) { set_err("null world"); return RB_ERR_INVALID; }
     int rc = validate_params(params);
     if (rc != RB_OK) return rc;
     // joint warm starting runs on the generic joint path, whose row tables are sized when the scene is set
     if (params->warmstart_joints && !W->w.generic_joints && !W->joints.empty()) {
-        set_err("warmstart_joints must be enabled before the scene is set%s", "");
+        set_err("warmstart_joints must be enabled before the scene is set");
         return RB_ERR_INVALID;
     }
     W->params = *params;
@@ -1324,27 +1360,36 @@ static int upload_joints(RbWorld* W) {
     return RB_OK;
 }
 
+static int validate_joint(const RbJointDesc& j, int nb, int index) {
+    if (j.body1 < 0 || j.body1 >= nb || j.body2 < 0 || j.body2 >= nb || (j.locked_axes & ~63u)) {
+        set_err("joint with bad body index or axes");
+        return RB_ERR_INVALID;
+    }
+    const unsigned ac = (j.coupled_axes >> 3) & 7u;   // limit_angular_coupled asserts exactly two coupled angular axes (joint_constraint_helper.rs:737-739)
+    if ((j.coupled_axes & ~63u) || (ac != 0 && ac != 3u && ac != 5u && ac != 6u)) {
+        set_err("joint %d: coupled_axes must couple exactly two angular axes (or none)", index);
+        return RB_ERR_INVALID;
+    }
+    return RB_OK;
+}
+
+// A limit or a motor on a free axis, or joint warm starting, needs the generic joint path (12 row slots per joint).
+// (Coupled axes only act through a limit or a motor.)
+static bool needs_generic_path(const RbWorld* W, const RbJointDesc& j) {
+    return ((j.limit_axes | j.motor_axes) & ~j.locked_axes & 63u) || W->params.warmstart_joints;
+}
+
 int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t nc, const RbColliderDesc* colliders,
                        int32_t nj, const RbJointDesc* joints) {
     if (!W || nb < 0 || nc < 0 || nj < 0 || (nb && !bodies) || (nc && !colliders) || (nj && !joints)) {
-        set_err("invalid scene arguments%s", "");
+        set_err("invalid scene arguments");
         return RB_ERR_INVALID;
     }
     CK(set_device(W->device));
     CK(stream_sync(W->stream));
     { int vrc = validate_descs(nb, nb, bodies, nc, colliders, (int)W->hulls.size()); if (vrc != RB_OK) return vrc; }
-    for (int i = 0; i < nj; ++i) {
-        const RbJointDesc& j = joints[i];
-        if (j.body1 < 0 || j.body1 >= nb || j.body2 < 0 || j.body2 >= nb || (j.locked_axes & ~63u)) {
-            set_err("joint with bad body index or axes%s", "");
-            return RB_ERR_INVALID;
-        }
-        const unsigned ac = (j.coupled_axes >> 3) & 7u;   // limit_angular_coupled asserts exactly two coupled angular axes (joint_constraint_helper.rs:737-739)
-        if ((j.coupled_axes & ~63u) || (ac != 0 && ac != 3u && ac != 5u && ac != 6u)) {
-            set_err("joint %s%d: coupled_axes must couple exactly two angular axes (or none)", "", i);
-            return RB_ERR_INVALID;
-        }
-    }
+    for (int i = 0; i < nj; ++i)
+        if (const int vrc = validate_joint(joints[i], nb, i); vrc != RB_OK) return vrc;
     W->steps_since_scene = 0;
     if (W->host_hint) W->host_hint[0] = W->host_hint[1] = W->host_hint[2] = W->host_hint[3] = 0;
     W->state_buf[0] = W->state_buf[1] = nullptr;
@@ -1356,6 +1401,7 @@ int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t
     if (rc != RB_OK) return rc;
 
     free_all(W);
+    W->wake_idx = nullptr; W->wake_cap = 0;
     World& w = W->w;
     W->force_events = false;
     W->ext_shapes = false;
@@ -1376,11 +1422,9 @@ int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t
     w.joint_cap = std::max(std::max(nj, W->reserve_joints), 1);
     w.item_cap = 4 + (NB + w.pair_cap + nj) / ITEM_TARGET;
     const int NJ = w.joint_cap;
-    w.generic_joints = ((nj > 0 && W->params.warmstart_joints) || W->reserve_generic) ? 1 : 0;   // joint warm starting: generic path too
-    for (int i = 0; i < nj; ++i) {   // any limit or motor on a free axis: the generic joint path (12 row slots per joint)
-        const unsigned free_axes = ~joints[i].locked_axes & 63u;
-        if ((joints[i].limit_axes | joints[i].motor_axes) & free_axes) w.generic_joints = 1;   // (coupled axes only act through a limit or a motor)
-    }
+    w.generic_joints = W->reserve_generic;
+    for (int i = 0; i < nj; ++i)
+        if (needs_generic_path(W, joints[i])) w.generic_joints = 1;
 
     ALLOC(w.st, 1);
     ALLOC(w.b_type, NB); ALLOC(w.b_flags, NB);
@@ -1498,40 +1542,24 @@ int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t
 // ---- incremental changes of the sets (src/pipeline/user_changes.rs:11-46, substep.rs:303-334) ----
 // Room for later rb_world_insert calls; takes effect at the next rb_world_set_scene.
 int rb_world_reserve(RbWorld* W, int32_t max_bodies, int32_t max_colliders) {
-    if (!W || max_bodies < 0 || max_colliders < 0) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || max_bodies < 0 || max_colliders < 0) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     W->reserve_bodies = max_bodies;
     W->reserve_colliders = max_colliders;
     return RB_OK;
 }
 
 int rb_world_reserve_joints(RbWorld* W, int32_t max_joints, int32_t generic) {
-    if (!W || max_joints < 0) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || max_joints < 0) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     W->reserve_joints = max_joints;
     W->reserve_generic = generic ? 1 : 0;
-    return RB_OK;
-}
-
-static int validate_joint(const RbJointDesc& j, int nb, int index) {
-    if (j.body1 < 0 || j.body1 >= nb || j.body2 < 0 || j.body2 >= nb || (j.locked_axes & ~63u)) {
-        set_err("joint with bad body index or axes%s", "");
-        return RB_ERR_INVALID;
-    }
-    const unsigned ac = (j.coupled_axes >> 3) & 7u;   // limit_angular_coupled asserts exactly two coupled angular axes (joint_constraint_helper.rs:737-739)
-    if ((j.coupled_axes & ~63u) || (ac != 0 && ac != 3u && ac != 5u && ac != 6u)) {
-        set_err("joint %s%d: coupled_axes must couple exactly two angular axes (or none)", "", index);
-        return RB_ERR_INVALID;
-    }
     return RB_OK;
 }
 
 // The joint set changed: colours, stage order and the contact-disabling pairs were recomputed (upload_joints); the islands and
 // the schedule follow at the next step, the broad phase re-filters its pairs.
 static int joints_changed(RbWorld* W) {
-    int one = 1;
-    CK(h2d(&W->w.st->bp_dirty, &one, sizeof(int)));
-    CK(h2d(&W->w.st->sched_dirty, &one, sizeof(int)));
     CK(h2d(&W->w.st->njused_colors, &W->njused, sizeof(int)));
-    return RB_OK;
+    return mark_dirty(W, 0, 1, 1);
 }
 
 // ImpulseJointSet::insert after the world has been uploaded (impulse_joint_set.rs; user_changes.rs): appended joints keep every
@@ -1539,15 +1567,14 @@ static int joints_changed(RbWorld* W) {
 // axes -- and any joint under warmstart_joints -- need the generic joint path, which a world without such joints only has when
 // it was reserved with generic = 1.
 int rb_world_insert_joints(RbWorld* W, int32_t n, const RbJointDesc* joints, int32_t* first_joint) {
-    if (!W || n < 0 || (n && !joints) || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || n < 0 || (n && !joints) || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     const int nj0 = W->w.nj;
-    if (nj0 + n > W->w.joint_cap) { set_err("rb_world_insert_joints exceeds the reserved capacity (rb_world_reserve_joints before rb_world_set_scene)%s", ""); return RB_ERR_CAPACITY; }
+    if (nj0 + n > W->w.joint_cap) { set_err("rb_world_insert_joints exceeds the reserved capacity (rb_world_reserve_joints before rb_world_set_scene)"); return RB_ERR_CAPACITY; }
     for (int i = 0; i < n; ++i) {
         int rc = validate_joint(joints[i], W->w.nb, nj0 + i);
         if (rc != RB_OK) return rc;
-        const unsigned free_axes = ~joints[i].locked_axes & 63u;
-        if ((((joints[i].limit_axes | joints[i].motor_axes) & free_axes) || W->params.warmstart_joints) && !W->w.generic_joints) {
-            set_err("this joint needs the generic joint path: reserve it with rb_world_reserve_joints(.., generic = 1)%s", "");
+        if (needs_generic_path(W, joints[i]) && !W->w.generic_joints) {
+            set_err("this joint needs the generic joint path: reserve it with rb_world_reserve_joints(.., generic = 1)");
             return RB_ERR_INVALID;
         }
     }
@@ -1568,9 +1595,9 @@ int rb_world_insert_joints(RbWorld* W, int32_t n, const RbJointDesc* joints, int
 // ImpulseJointSet::remove: the slot stays allocated (indices of the other joints are unchanged), the joint is neither solved
 // nor an island edge any more, and contacts it disabled come back.
 int rb_world_remove_joints(RbWorld* W, int32_t n, const int32_t* indices) {
-    if (!W || n < 0 || (n && !indices) || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || n < 0 || (n && !indices) || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     for (int k = 0; k < n; ++k)
-        if (indices[k] < 0 || indices[k] >= W->w.nj) { set_err("joint index out of range%s", ""); return RB_ERR_INVALID; }
+        if (indices[k] < 0 || indices[k] >= W->w.nj) { set_err("joint index out of range"); return RB_ERR_INVALID; }
     int rc = sync_world(W);
     if (rc != RB_OK) return rc;
     W->joint_removed.resize(W->joints.size(), 0);
@@ -1582,7 +1609,7 @@ int rb_world_remove_joints(RbWorld* W, int32_t n, const int32_t* indices) {
 // Registers a convex polyhedron (closed convex mesh: vertices + polygonal faces) that RB_SHAPE_CONVEX colliders refer to
 // by the id returned (>= 1; 0 is the unit cube).  Negative = RB_ERR_*.  Hulls persist across rb_world_set_scene.
 int32_t rb_world_add_hull(RbWorld* W, int32_t nv, const float* verts, int32_t nf, const int32_t* face_sizes, const int32_t* face_indices) {
-    if (!W || !verts || !face_sizes || !face_indices) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || !verts || !face_sizes || !face_indices) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     rbhull::Hull h;
     const char* why = rbhull::from_mesh(nv, verts, nf, face_sizes, face_indices, h);
     if (why) { set_err("convex mesh rejected: %s", why); return RB_ERR_INVALID; }
@@ -1593,7 +1620,7 @@ int32_t rb_world_add_hull(RbWorld* W, int32_t nv, const float* verts, int32_t nf
 // ColliderBuilder::convex_hull's hull computation (parry transformation::convex_hull) for at most 32 points: writes the
 // hull's vertices (a subset of the points, in input order), face sizes and face vertex indices.  Host code only.
 int32_t rb_convex_hull(int32_t npoints, const float* points, int32_t* nv, float* verts, int32_t* nf, int32_t* face_sizes, int32_t* face_indices) {
-    if (!points || !nv || !verts || !nf || !face_sizes || !face_indices) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!points || !nv || !verts || !nf || !face_sizes || !face_indices) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     std::vector<float> v;
     std::vector<int32_t> sizes, idx;
     const char* why = rbhull::convex_hull(npoints, points, v, sizes, idx);
@@ -1610,22 +1637,21 @@ int32_t rb_convex_hull(int32_t npoints, const float* points, int32_t* nv, float*
 // New colliders may only be attached to the new bodies (or to none).  Joints cannot be inserted this way.
 int rb_world_insert(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t nc, const RbColliderDesc* colliders,
                     int32_t* first_body, int32_t* first_collider) {
-    if (!W || nb < 0 || nc < 0 || (nb && !bodies) || (nc && !colliders) || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || nb < 0 || nc < 0 || (nb && !bodies) || (nc && !colliders) || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     const int nb0 = W->w.nb, nc0 = W->w.nc;
     if (nb0 + nb > W->body_cap || nc0 + nc > W->collider_cap) {
-        set_err("rb_world_insert exceeds the reserved capacity (rb_world_reserve before rb_world_set_scene)%s", "");
+        set_err("rb_world_insert exceeds the reserved capacity (rb_world_reserve before rb_world_set_scene)");
         return RB_ERR_CAPACITY;
     }
     int rc = validate_descs(nb0 + nb, nb, bodies, nc, colliders, (int)W->hulls.size());
     if (rc != RB_OK) return rc;
     for (int i = 0; i < nc; ++i)
-        if (colliders[i].parent >= 0 && colliders[i].parent < nb0) { set_err("new colliders may only be attached to new bodies%s", ""); return RB_ERR_INVALID; }
-    rc = sync_world(W);
-    if (rc != RB_OK) return rc;
+        if (colliders[i].parent >= 0 && colliders[i].parent < nb0) { set_err("new colliders may only be attached to new bodies"); return RB_ERR_INVALID; }
     W->bodies.insert(W->bodies.end(), bodies, bodies + nb);
     W->colliders.insert(W->colliders.end(), colliders, colliders + nc);
     std::vector<HostMass> mp;
-    rc = host_mass_props(W, mp, nb0, nc0);
+    rc = host_mass_props(W, mp, nb0, nc0);   // (may reject the new bodies' mass properties: before anything is waited on or written)
+    if (rc == RB_OK) rc = sync_world(W);
     if (rc != RB_OK) { W->bodies.resize(nb0); W->colliders.resize(nc0); return rc; }
     W->w.nb = nb0 + nb;
     W->w.nc = nc0 + nc;
@@ -1633,12 +1659,10 @@ int rb_world_insert(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t nc
     if ((rc = upload_hulls(W)) != RB_OK) return rc;
     if ((rc = upload_bodies(W, mp, nb0, nb)) != RB_OK) return rc;
     if ((rc = upload_colliders(W, nc0, nc, nb0)) != RB_OK) return rc;
-    int one = 1, lists = 1;   // lists: 1 = only movers were added, 3 = static colliders too (re-sort them)
+    int lists = 1;   // 1 = only movers were added, 3 = static colliders too (re-sort them)
     for (int i = 0; i < nc; ++i)
         if (colliders[i].parent < 0 || !type_moves(W->bodies[colliders[i].parent].body_type)) lists = 3;
-    CK(h2d(&W->w.st->lists_dirty, &lists, sizeof(int)));
-    CK(h2d(&W->w.st->bp_dirty, &one, sizeof(int)));
-    CK(h2d(&W->w.st->sched_dirty, &one, sizeof(int)));
+    if ((rc = mark_dirty(W, lists, 1, 1)) != RB_OK) return rc;
     if (first_body) *first_body = nb0;
     if (first_collider) *first_collider = nc0;
     rc = launch_init_bodies(W, nb0);
@@ -1650,11 +1674,10 @@ int rb_world_insert(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t nc
 // allocated (indices of everything else are unchanged), the colliders leave the broad phase, so their contact
 // pairs end at the next step.
 int rb_world_remove_bodies(RbWorld* W, int32_t n, const int32_t* indices) {
-    if (!W || n < 0 || (n && !indices) || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
-    int rc = sync_world(W);
+    if (!W || n < 0 || (n && !indices) || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
+    int rc = check_bodies(W, n, indices);
+    if (rc == RB_OK) rc = sync_world(W);
     if (rc != RB_OK) return rc;
-    for (int k = 0; k < n; ++k)
-        if (indices[k] < 0 || indices[k] >= W->w.nb) { set_err("body index out of range%s", ""); return RB_ERR_INVALID; }
     const int removed_type = BODY_REMOVED, removed_shape = SHAPE_REMOVED;
     for (int k = 0; k < n; ++k) {
         const int b = indices[k];
@@ -1663,10 +1686,7 @@ int rb_world_remove_bodies(RbWorld* W, int32_t n, const int32_t* indices) {
         for (int c = 0; c < (int)W->colliders.size(); ++c)
             if (W->colliders[c].parent == b) CK(h2d(W->w.c_shape + c, &removed_shape, sizeof(int)));
     }
-    int one = 1, lists = 3;
-    CK(h2d(&W->w.st->lists_dirty, &lists, sizeof(int)));
-    CK(h2d(&W->w.st->bp_dirty, &one, sizeof(int)));
-    CK(h2d(&W->w.st->sched_dirty, &one, sizeof(int)));
+    if ((rc = mark_dirty(W, 3, 1, 1)) != RB_OK) return rc;
     return wake_impl(W, nullptr, 0);   // (the reference wakes what touched the removed body; here: everything asleep)
 }
 
@@ -1699,24 +1719,11 @@ int rb_world_get_sleeping(RbWorld* W, uint8_t* sleeping) {
     return RB_OK;
 }
 
-static int wake_impl(RbWorld* W, const int32_t* indices_host, int n) {
-    int* idx_dev = nullptr;
-    if (indices_host) {
-        if (dev_alloc((void**)&idx_dev, (size_t)std::max(n, 1) * sizeof(int)) != cudaSuccess) { set_err("device allocation failed%s", ""); return RB_ERR_CUDA; }
-        CK(h2d(idx_dev, indices_host, (size_t)n * sizeof(int)));
-    }
-    CK(set_device(W->device));
-    const int work = indices_host ? n : W->w.nb;
-    CK(launch(W, k_wake, (std::max(work, 1) + 255) / 256, 256, 0, false, W->w, idx_dev, n));
-    if (indices_host) CK(launch(W, k_wake_apply, (std::max(W->w.nb, 1) + 255) / 256, 256, 0, false, W->w));
-    CK(stream_sync(W->stream));
-    if (idx_dev) dev_free(idx_dev);
-    return RB_OK;
-}
 // RigidBody::wake_up(strong = true) through IslandManager::wake_up: the bodies' whole islands.
 int rb_world_wake_up(RbWorld* W, int32_t n, const int32_t* indices) {
-    if (!W || n < 0 || (n && !indices) || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
-    if (n == 0) return RB_OK;
+    if (!W || n < 0 || (n && !indices) || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
+    const int rc = check_bodies(W, n, indices);
+    if (rc != RB_OK || n == 0) return rc;
     return wake_impl(W, indices, n);
 }
 
@@ -1724,20 +1731,19 @@ int rb_world_wake_up(RbWorld* W, int32_t n, const int32_t* indices) {
 // listed joints take the new descriptors in place.  Their bodies must stay the same (otherwise remove + insert); impulses carried
 // for warm starting are kept; with wake_up the islands of the attached bodies are woken (issue_692_joint_get_mut_wakes_bodies.rs).
 int rb_world_update_joints(RbWorld* W, int32_t n, const int32_t* indices, const RbJointDesc* joints, int32_t wake_up) {
-    if (!W || n < 0 || (n && (!indices || !joints)) || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || n < 0 || (n && (!indices || !joints)) || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     W->joint_removed.resize(W->joints.size(), 0);
     for (int k = 0; k < n; ++k) {
         const int i = indices[k];
-        if (i < 0 || i >= W->w.nj || W->joint_removed[i]) { set_err("joint index out of range (or removed)%s", ""); return RB_ERR_INVALID; }
+        if (i < 0 || i >= W->w.nj || W->joint_removed[i]) { set_err("joint index out of range (or removed)"); return RB_ERR_INVALID; }
         int rc = validate_joint(joints[k], W->w.nb, i);
         if (rc != RB_OK) return rc;
         if (joints[k].body1 != W->joints[i].body1 || joints[k].body2 != W->joints[i].body2) {
-            set_err("rb_world_update_joints cannot move a joint to other bodies: remove it and insert a new one%s", "");
+            set_err("rb_world_update_joints cannot move a joint to other bodies: remove it and insert a new one");
             return RB_ERR_INVALID;
         }
-        const unsigned free_axes = ~joints[k].locked_axes & 63u;
-        if (((joints[k].limit_axes | joints[k].motor_axes) & free_axes) && !W->w.generic_joints) {
-            set_err("this joint needs the generic joint path: reserve it with rb_world_reserve_joints(.., generic = 1)%s", "");
+        if (needs_generic_path(W, joints[k]) && !W->w.generic_joints) {
+            set_err("this joint needs the generic joint path: reserve it with rb_world_reserve_joints(.., generic = 1)");
             return RB_ERR_INVALID;
         }
     }
@@ -1756,12 +1762,12 @@ int rb_world_update_joints(RbWorld* W, int32_t n, const int32_t* indices, const 
 }
 
 int rb_world_set_body_states(RbWorld* W, int32_t n, const int32_t* indices, const float* pose7, const float* vel6) {
-    if (!W || n < 0 || (n && !indices)) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
-    int rc = sync_world(W);
+    if (!W || n < 0 || (n && !indices)) { set_err("invalid arguments"); return RB_ERR_INVALID; }
+    int rc = check_bodies(W, n, indices);
+    if (rc == RB_OK) rc = sync_world(W);
     if (rc != RB_OK) return rc;
     for (int k = 0; k < n; ++k) {
-        int i = indices[k];
-        if (i < 0 || i >= W->w.nb) { set_err("body index out of range%s", ""); return RB_ERR_INVALID; }
+        const int i = indices[k];
         if (pose7) {
             float4 t = make_float4(pose7[k * 7], pose7[k * 7 + 1], pose7[k * 7 + 2], 0.f);
             float4 q = make_float4(pose7[k * 7 + 3], pose7[k * 7 + 4], pose7[k * 7 + 5], pose7[k * 7 + 6]);
@@ -1777,16 +1783,9 @@ int rb_world_set_body_states(RbWorld* W, int32_t n, const int32_t* indices, cons
             CK(h2d(W->w.b_angvel + i, &a, sizeof(a)));
         }
     }
-    {   // a teleported FIXED body moves static colliders: rebuild the broad-phase lists (and re-sort the static ones)
-        bool moved_static = false;
-        if (pose7)
-            for (int k = 0; k < n; ++k) moved_static = moved_static || !type_moves(W->bodies[indices[k]].body_type);
-        if (moved_static) {
-            int one = 1, lists = 3;
-            CK(h2d(&W->w.st->lists_dirty, &lists, sizeof(int)));
-            CK(h2d(&W->w.st->bp_dirty, &one, sizeof(int)));
-        }
-    }
+    bool moved_static = false;   // a teleported FIXED body moves static colliders: rebuild the broad-phase lists (and re-sort the static ones)
+    for (int k = 0; pose7 && k < n; ++k) moved_static = moved_static || !type_moves(W->bodies[indices[k]].body_type);
+    if (moved_static && (rc = mark_dirty(W, 3, 1, 0)) != RB_OK) return rc;
     rc = launch_init_bodies(W);
     if (rc != RB_OK) return rc;
     if (n > 0 && (rc = wake_impl(W, indices, n)) != RB_OK) return rc;   // a user change wakes the body's island (user_changes.rs)
@@ -1794,12 +1793,12 @@ int rb_world_set_body_states(RbWorld* W, int32_t n, const int32_t* indices, cons
 }
 
 int rb_world_set_body_forces(RbWorld* W, int32_t n, const int32_t* indices, const float* force3, const float* torque3) {
-    if (!W || n < 0 || (n && !indices)) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
-    int rc = sync_world(W);
+    if (!W || n < 0 || (n && !indices)) { set_err("invalid arguments"); return RB_ERR_INVALID; }
+    int rc = check_bodies(W, n, indices);
+    if (rc == RB_OK) rc = sync_world(W);
     if (rc != RB_OK) return rc;
     for (int k = 0; k < n; ++k) {
         const int i = indices[k];
-        if (i < 0 || i >= W->w.nb) { set_err("body index out of range%s", ""); return RB_ERR_INVALID; }
         if (force3) {
             float4 f = make_float4(force3[k * 3], force3[k * 3 + 1], force3[k * 3 + 2], 0.f);
             CK(h2d(W->w.b_uforce + i, &f, sizeof(f)));
@@ -1816,15 +1815,13 @@ int rb_world_set_body_forces(RbWorld* W, int32_t n, const int32_t* indices, cons
 }
 
 int rb_world_set_next_kinematic_positions(RbWorld* W, int32_t n, const int32_t* indices, const float* pose7) {
-    if (!W || n < 0 || (n && (!indices || !pose7))) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
-    int rc = sync_world(W);
+    if (!W || n < 0 || (n && (!indices || !pose7))) { set_err("invalid arguments"); return RB_ERR_INVALID; }
+    int rc = check_bodies(W, n, indices, "rb_world_set_next_kinematic_positions: not a position-based kinematic body",
+                          RB_BODY_KINEMATIC_POSITION_BASED);
+    if (rc == RB_OK) rc = sync_world(W);
     if (rc != RB_OK) return rc;
     for (int k = 0; k < n; ++k) {
         const int i = indices[k];
-        if (i < 0 || i >= W->w.nb || W->bodies[i].body_type != RB_BODY_KINEMATIC_POSITION_BASED) {
-            set_err("rb_world_set_next_kinematic_positions: not a position-based kinematic body%s", "");
-            return RB_ERR_INVALID;
-        }
         float4 t = make_float4(pose7[k * 7], pose7[k * 7 + 1], pose7[k * 7 + 2], 0.f);
         float4 q = make_float4(pose7[k * 7 + 3], pose7[k * 7 + 4], pose7[k * 7 + 5], pose7[k * 7 + 6]);
         CK(h2d(W->w.b_next_t + i, &t, sizeof(t)));
@@ -1835,7 +1832,7 @@ int rb_world_set_next_kinematic_positions(RbWorld* W, int32_t n, const int32_t* 
 }
 
 int rb_world_drain_collision_events(RbWorld* W, int32_t cap, RbCollisionEvent* out) {
-    if (!W || cap < 0 || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || cap < 0 || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     State st;
     int rc = read_state(W, st);
     if (rc != RB_OK) return rc;
@@ -1857,7 +1854,7 @@ int rb_world_drain_collision_events(RbWorld* W, int32_t cap, RbCollisionEvent* o
 }
 
 int rb_world_drain_contact_force_events(RbWorld* W, int32_t cap, RbContactForceEvent* out) {
-    if (!W || cap < 0 || !W->w.st) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || cap < 0 || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     State st;
     int rc = read_state(W, st);
     if (rc != RB_OK) return rc;
@@ -1885,7 +1882,7 @@ int rb_world_drain_contact_force_events(RbWorld* W, int32_t cap, RbContactForceE
 }
 
 int rb_world_step(RbWorld* W, const float gravity[3], int32_t nsteps, int32_t sync) {
-    if (!W || !gravity || nsteps < 0) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!W || !gravity || nsteps < 0) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     if (W->w.nb == 0 && W->w.nc == 0) return RB_OK;
     Grav g{gravity[0], gravity[1], gravity[2]};
     CK(set_device(W->device));
@@ -2078,7 +2075,8 @@ int64_t rb_world_debug_read(RbWorld* W, const char* table, void* dst, int64_t ca
         for (int i = 0; i < n; ++i) put(&r[i], 12);
     } else if (t == "pair_points") {
         std::vector<float4> pa, pb, pd;
-        if (n > 0) { fetch_rows(W, st, PR_PA, MAX_PTS, pa); fetch_rows(W, st, PR_PB, MAX_PTS, pb); fetch_rows(W, st, PR_PD, MAX_PTS, pd); }
+        if (n > 0 && ((rc = fetch_rows(W, st, PR_PA, MAX_PTS, pa)) != RB_OK || (rc = fetch_rows(W, st, PR_PB, MAX_PTS, pb)) != RB_OK ||
+                      (rc = fetch_rows(W, st, PR_PD, MAX_PTS, pd)) != RB_OK)) return rc;
         for (int i = 0; i < n; ++i)
             for (int k = 0; k < 4; ++k) {
                 float rec[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -2090,7 +2088,8 @@ int64_t rb_world_debug_read(RbWorld* W, const char* table, void* dst, int64_t ca
             }
     } else if (t == "pair_data") {
         std::vector<float4> pd, tw, d1, d2;
-        if (n > 0) { fetch_rows(W, st, PR_PD, MAX_PTS, pd); fetch_rows(W, st, PR_TW, MAX_PTS, tw); fetch_rows(W, st, PR_DP1, MAX_PTS, d1); fetch_rows(W, st, PR_DP2, MAX_PTS, d2); }
+        if (n > 0 && ((rc = fetch_rows(W, st, PR_PD, MAX_PTS, pd)) != RB_OK || (rc = fetch_rows(W, st, PR_TW, MAX_PTS, tw)) != RB_OK ||
+                      (rc = fetch_rows(W, st, PR_DP1, MAX_PTS, d1)) != RB_OK || (rc = fetch_rows(W, st, PR_DP2, MAX_PTS, d2)) != RB_OK)) return rc;
         for (int i = 0; i < n; ++i)
             for (int k = 0; k < 4; ++k) {
                 float rec[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -2103,7 +2102,7 @@ int64_t rb_world_debug_read(RbWorld* W, const char* table, void* dst, int64_t ca
             }
     } else if (t == "pair_sc") {
         std::vector<float4> a1, a2;
-        if (n > 0) { fetch_rows(W, st, PR_A1, MAX_PTS, a1); fetch_rows(W, st, PR_A2, MAX_PTS, a2); }
+        if (n > 0 && ((rc = fetch_rows(W, st, PR_A1, MAX_PTS, a1)) != RB_OK || (rc = fetch_rows(W, st, PR_A2, MAX_PTS, a2)) != RB_OK)) return rc;
         for (int i = 0; i < n; ++i)
             for (int k = 0; k < 4; ++k) {
                 float rec[6] = {0, 0, 0, 0, 0, 0};
@@ -2201,7 +2200,7 @@ int64_t rb_world_debug_read(RbWorld* W, const char* table, void* dst, int64_t ca
 
 // Unit-level known-answer entry point (parity tests): evaluates one device function on literal inputs.
 int rb_debug_kat(const char* name, const float* in, int32_t n_in, float* out, int32_t n_out) {
-    if (!name || !in || !out || n_in <= 0 || n_out <= 0) { set_err("invalid arguments%s", ""); return RB_ERR_INVALID; }
+    if (!name || !in || !out || n_in <= 0 || n_out <= 0) { set_err("invalid arguments"); return RB_ERR_INVALID; }
     static const struct { const char* n; int id, nin, nout; } T[] = {
         {"pose_drift", KAT_POSE_DRIFT, 15, 1}, {"reduce_manifold", KAT_REDUCE, 5, 5}, {"normal_solve", KAT_NORMAL_SOLVE, 37, 13},
         {"tangent_solve", KAT_TANGENT_SOLVE, 59, 14}, {"generate", KAT_GENERATE, 25, 39}, {"ccd_toi", KAT_CCD_TOI, 33, 1},
@@ -2243,12 +2242,11 @@ int rb_world_label_components(RbWorld* W, int32_t* component_of_body) {
     if (!W || !component_of_body) return RB_ERR_INVALID;
     // Run the collision pipeline once (it leaves poses untouched) so the island labels are current.
     CK(set_device(W->device));
-    int one = 1;
     CK(stream_sync(W->stream));
-    CK(h2d(&W->w.st->sched_dirty, &one, sizeof(int)));
-    CK(launch(W, W->ext_shapes ? k_collide<1> : k_collide<0>, W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, true, W->w, Grav{0.f, 0.f, 0.f}, 0));
-    int rc = sync_world(W);
+    int rc = mark_dirty(W, 0, 0, 1);
     if (rc != RB_OK) return rc;
+    CK(launch(W, W->ext_shapes ? k_collide<1> : k_collide<0>, W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, true, W->w, Grav{0.f, 0.f, 0.f}, 0));
+    if ((rc = sync_world(W)) != RB_OK) return rc;
     CK(d2h(component_of_body, W->w.isl_label, (size_t)W->w.nb * sizeof(int)));
     for (int i = 0; i < W->w.nb; ++i)
         if (!type_moves(W->bodies[i].body_type)) component_of_body[i] = -1;
@@ -2258,7 +2256,7 @@ int rb_world_label_components(RbWorld* W, int32_t* component_of_body) {
 int rb_world_set_owned_bodies(RbWorld* W, const uint8_t* owned) {
     if (!W || !owned) return RB_ERR_INVALID;
     if (W->steps > 0) {   // the partition drops the pair table (warm start, colours): only before the first step
-        set_err("rb_world_set_owned_bodies must be called before the world is stepped%s", "");
+        set_err("rb_world_set_owned_bodies must be called before the world is stepped");
         return RB_ERR_INVALID;
     }
     int rc = sync_world(W);
