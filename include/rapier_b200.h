@@ -12,9 +12,9 @@
  * memory; the library copies.  One RbWorld is not re-entrant (the reference takes `&mut self`).
  * Every function returns RB_OK (0) or a negative RbStatus; rb_last_error() describes the failure.
  * The calls that edit the sets -- rb_world_set_body_states, rb_world_set_body_forces, rb_world_set_next_kinematic_positions,
- * rb_world_wake_up, rb_world_insert, rb_world_remove_bodies, rb_world_insert_joints, rb_world_remove_joints and
- * rb_world_update_joints -- check all of their input before they change anything: a call that returns RB_ERR_INVALID
- * has applied none of its entries and woken no body.
+ * rb_world_wake_up, rb_world_insert, rb_world_remove_bodies, rb_world_insert_joints, rb_world_remove_joints,
+ * rb_world_update_joints and rb_world_set_collider_filters -- check all of their input before they change anything: a call
+ * that returns RB_ERR_INVALID has applied none of its entries and woken no body.
  * There is NO CPU fallback: without a CUDA device rb_world_create fails with RB_ERR_NO_DEVICE.
  */
 #ifndef RAPIER_B200_H
@@ -141,6 +141,33 @@ typedef struct RbColliderDesc {
                                         * are tested for intersection only (narrow_phase/intersections.rs) and report CollisionEvents
                                         * carrying RB_COLLISION_EVENT_SENSOR; it still counts for the mass of its body.  Default 0. */
 } RbColliderDesc;
+
+/* ActiveCollisionTypes (src/geometry/collider_components.rs:282-345): which pairs of body types a collider may collide with.
+ * A pair is kept when either collider's bits allow the pair's two body types (a parentless collider counts as fixed).  The
+ * RB_BODY_* numbers are the reference's RigidBodyType values, so its bit layout applies unchanged. */
+enum {
+    RB_ACT_DYNAMIC_DYNAMIC = 0x0001, RB_ACT_DYNAMIC_KINEMATIC = 0x000C, RB_ACT_DYNAMIC_FIXED = 0x0002,
+    RB_ACT_KINEMATIC_KINEMATIC = 0xCC00, RB_ACT_KINEMATIC_FIXED = 0x2200, RB_ACT_FIXED_FIXED = 0x0020,
+    RB_ACT_DEFAULT = 0x000F   /* DYNAMIC_DYNAMIC | DYNAMIC_KINEMATIC | DYNAMIC_FIXED */
+};
+/* InteractionTestMode (src/geometry/interaction_groups.rs:74-154): And needs memberships1 & filter2 and memberships2 & filter1;
+ * Or needs either, and applies only when BOTH colliders use it. */
+enum { RB_TEST_AND = 0, RB_TEST_OR = 1 };
+/* The filters of one collider (ColliderFlags, collider_components.rs:363-379).
+ *   collision_*: InteractionGroups of the broad / narrow phase (Collider::set_collision_groups): a pair that fails has no contact
+ *                and no event.
+ *   solver_*:    InteractionGroups of the solver (Collider::set_solver_groups): a pair that fails keeps its contacts and its
+ *                CollisionEvents but computes no force.
+ *   active_collision_types: RB_ACT_* bits (Collider::set_active_collision_types).
+ * Every collider starts with collision groups from its RbColliderDesc (And mode), solver groups all() in And mode and
+ * RB_ACT_DEFAULT. */
+typedef struct RbColliderFilter {
+    uint32_t collision_memberships, collision_filter;
+    int32_t collision_test_mode;       /* RB_TEST_* */
+    uint32_t solver_memberships, solver_filter;
+    int32_t solver_test_mode;          /* RB_TEST_* */
+    uint32_t active_collision_types;   /* RB_ACT_* */
+} RbColliderFilter;
 
 /* ActiveEvents (src/pipeline/event_handler.rs). */
 enum { RB_EVENT_COLLISION = 1, RB_EVENT_CONTACT_FORCE = 2 };
@@ -289,6 +316,15 @@ int rb_world_remove_joints(RbWorld* w, int32_t n, const int32_t* joint_indices);
  * frames, softness ...).  Bodies must stay the same; warm-start impulses are kept; wake_up != 0 wakes the attached bodies'
  * islands (crates/rapier3d/tests/issue_692_joint_get_mut_wakes_bodies.rs). */
 int rb_world_update_joints(RbWorld* w, int32_t n, const int32_t* joint_indices, const RbJointDesc* joints, int32_t wake_up);
+/* Collider::set_collision_groups / set_solver_groups / set_active_collision_types: collider_indices[k] takes filters[k].  Takes
+ * effect at the next step: a pair the new filters forbid leaves the pair set (a touching one emits a Stopped event), a pair
+ * they allow is found by the broad phase, a pair whose solver groups now fail (or pass) is recomputed in full, and every other
+ * pair keeps its contacts and warm-start impulses.  The bodies of the changed colliders and of every collider they share a pair
+ * with are woken.  Pairs of two static colliders (RB_ACT_FIXED_FIXED) are searched for when a static collider's filters
+ * change; more of them than the pair capacity raise RB_ERR_CAPACITY at the next step.
+ * RB_ERR_INVALID: an index out of range or of a removed collider, a test mode other than RB_TEST_AND / RB_TEST_OR, or a
+ * collision-type bit outside RB_ACT_*. */
+int rb_world_set_collider_filters(RbWorld* w, int32_t n, const int32_t* collider_indices, const RbColliderFilter* filters);
 
 /* ---- convex polyhedra (ColliderBuilder::{convex_hull, convex_mesh, round_convex_hull}, src/geometry/collider.rs:1039-1090;
  *      parry ConvexPolyhedron) ----

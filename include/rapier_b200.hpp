@@ -102,8 +102,20 @@ public:
     ColliderBuilder& restitution_combine_rule(int r) { d_.restitution_combine_rule = r; return *this; }
     ColliderBuilder& translation(Vector v) { for (int i = 0; i < 3; ++i) d_.pos_wrt_parent_t[i] = v[i]; return *this; }
     ColliderBuilder& contact_skin(float x) { d_.contact_skin = x; return *this; }
-    ColliderBuilder& collision_groups(unsigned memberships, unsigned filter) {
-        d_.collision_memberships = memberships; d_.collision_filter = filter; return *this;
+    ColliderBuilder& collision_groups(unsigned memberships, unsigned filter, int test_mode = RB_TEST_AND) {   // RB_TEST_*
+        d_.collision_memberships = memberships; d_.collision_filter = filter; f_.collision_test_mode = test_mode; return *this;
+    }
+    // ColliderBuilder::solver_groups / active_collision_types (RbColliderFilter, applied by PhysicsPipeline after the upload)
+    ColliderBuilder& solver_groups(unsigned memberships, unsigned filter, int test_mode = RB_TEST_AND) {
+        f_.solver_memberships = memberships; f_.solver_filter = filter; f_.solver_test_mode = test_mode; return *this;
+    }
+    ColliderBuilder& active_collision_types(unsigned bits) { f_.active_collision_types = bits; return *this; }   // RB_ACT_*
+    // The collider's filters; false when everything but the collision groups (which the descriptor carries) is the default.
+    bool filter(RbColliderFilter& out) const {
+        out = f_;
+        out.collision_memberships = d_.collision_memberships; out.collision_filter = d_.collision_filter;
+        return f_.collision_test_mode != RB_TEST_AND || f_.solver_memberships != 0xffffffffu || f_.solver_filter != 0xffffffffu ||
+               f_.solver_test_mode != RB_TEST_AND || f_.active_collision_types != RB_ACT_DEFAULT;
     }
     ColliderBuilder& active_events(unsigned events) { d_.active_events = events; return *this; }   // RB_EVENT_*
     ColliderBuilder& contact_force_event_threshold(float t) { d_.contact_force_event_threshold = t; return *this; }
@@ -119,8 +131,10 @@ private:
         d_.density = 1.0f; d_.friction = 0.5f; d_.restitution = 0.0f;           // collider.rs:688-707
         d_.friction_combine_rule = RB_COMBINE_AVERAGE; d_.restitution_combine_rule = RB_COMBINE_AVERAGE;
         d_.collision_memberships = 0xffffffffu; d_.collision_filter = 0xffffffffu;
+        f_ = RbColliderFilter{0xffffffffu, 0xffffffffu, RB_TEST_AND, 0xffffffffu, 0xffffffffu, RB_TEST_AND, RB_ACT_DEFAULT};
     }
     RbColliderDesc d_;
+    RbColliderFilter f_;
 };
 
 // GenericJoint / GenericJointBuilder (src/dynamics/joint/generic_joint.rs): locked axes, limits and motors on the free
@@ -199,10 +213,17 @@ struct RigidBodySet {
 };
 struct ColliderSet {
     std::vector<RbColliderDesc> colliders;
+    std::vector<int32_t> filtered;              // colliders whose filters are not the defaults ...
+    std::vector<RbColliderFilter> filters;      // ... and those filters
     bool modified = true;
-    ColliderHandle insert(const ColliderBuilder& c) { colliders.push_back(c.desc(-1)); modified = true; return {int(colliders.size()) - 1}; }
-    ColliderHandle insert_with_parent(const ColliderBuilder& c, RigidBodyHandle parent, RigidBodySet&) {
-        colliders.push_back(c.desc(parent.index)); modified = true; return {int(colliders.size()) - 1};
+    ColliderHandle insert(const ColliderBuilder& c) { return add(c, -1); }
+    ColliderHandle insert_with_parent(const ColliderBuilder& c, RigidBodyHandle parent, RigidBodySet&) { return add(c, parent.index); }
+    ColliderHandle add(const ColliderBuilder& c, int parent) {
+        colliders.push_back(c.desc(parent));
+        RbColliderFilter f;
+        if (c.filter(f)) { filtered.push_back(int(colliders.size()) - 1); filters.push_back(f); }
+        modified = true;
+        return {int(colliders.size()) - 1};
     }
     size_t len() const { return colliders.size(); }
 };
@@ -234,6 +255,8 @@ public:
         if (bodies.modified || colliders.modified || joints.modified) {   // handle_user_changes (substep.rs:303-334)
             check(rb_world_set_scene(w_, int(bodies.bodies.size()), bodies.bodies.data(), int(colliders.colliders.size()),
                                      colliders.colliders.data(), int(joints.joints.size()), joints.joints.data()));
+            if (!colliders.filtered.empty())
+                check(rb_world_set_collider_filters(w_, int(colliders.filtered.size()), colliders.filtered.data(), colliders.filters.data()));
             bodies.modified = colliders.modified = joints.modified = false;
         }
         check(rb_world_step(w_, gravity.data(), nsteps, sync ? 1 : 0));

@@ -102,6 +102,25 @@ class RbContactForceEvent(C.Structure):
 RB_EVENT_COLLISION, RB_EVENT_CONTACT_FORCE = 1, 2
 RB_COLLISION_EVENT_SENSOR = 1   # CollisionEventFlags::SENSOR
 
+# ActiveCollisionTypes (collider_components.rs:282-345) and InteractionTestMode (interaction_groups.rs:74-154)
+RB_ACT_DYNAMIC_DYNAMIC = 0x0001
+RB_ACT_DYNAMIC_KINEMATIC = 0x000C
+RB_ACT_DYNAMIC_FIXED = 0x0002
+RB_ACT_KINEMATIC_KINEMATIC = 0xCC00
+RB_ACT_KINEMATIC_FIXED = 0x2200
+RB_ACT_FIXED_FIXED = 0x0020
+RB_ACT_DEFAULT = 0x000F
+RB_TEST_AND, RB_TEST_OR = 0, 1
+
+
+class RbColliderFilter(C.Structure):
+    """The filters of one collider (ColliderFlags, collider_components.rs:363-379)."""
+    _fields_ = [
+        ("collision_memberships", u32), ("collision_filter", u32), ("collision_test_mode", i32),
+        ("solver_memberships", u32), ("solver_filter", u32), ("solver_test_mode", i32),
+        ("active_collision_types", u32),
+    ]
+
 
 class RbJointMotor(C.Structure):
     _fields_ = [("target_vel", f32), ("target_pos", f32), ("stiffness", f32), ("damping", f32), ("max_force", f32), ("model", i32)]

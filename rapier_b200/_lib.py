@@ -24,6 +24,7 @@ EXPORTS = [
     "rb_world_debug_read", "rb_world_label_components", "rb_world_set_owned_bodies",
     "rb_world_state_buffer", "rb_world_import_states", "rb_world_import_states_from", "rb_world_state_buffers", "rb_world_stream", "rb_world_set_stream",
     "rb_world_step_host", "rb_debug_kat", "rb_world_get_quarantine", "rb_world_get_sleeping", "rb_world_wake_up", "rb_world_set_halo_bodies", "rb_world_import_halo", "rb_world_reserve", "rb_world_insert", "rb_world_remove_bodies", "rb_world_reserve_joints", "rb_world_insert_joints", "rb_world_remove_joints", "rb_world_update_joints",
+    "rb_world_set_collider_filters",
     "rb_world_set_body_forces", "rb_world_set_next_kinematic_positions", "rb_world_drain_collision_events", "rb_world_drain_contact_force_events",
     "rb_world_add_hull", "rb_convex_hull",
 ]
@@ -72,6 +73,7 @@ def declare(L):
     L.rb_world_insert_joints.argtypes = [vp, i32, vp, vp]
     L.rb_world_remove_joints.argtypes = [vp, i32, vp]
     L.rb_world_update_joints.argtypes = [vp, i32, vp, vp, i32]
+    L.rb_world_set_collider_filters.argtypes = [vp, i32, vp, vp]
     L.rb_world_set_body_forces.argtypes = [vp, i32, vp, vp, vp]
     L.rb_world_set_next_kinematic_positions.argtypes = [vp, i32, vp, vp]
     L.rb_world_drain_collision_events.argtypes = [vp, i32, vp]

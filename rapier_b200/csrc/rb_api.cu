@@ -494,6 +494,7 @@ struct RbWorld {
     float* stage_dev = nullptr;      // [nb*13] device staging for bulk state import
     int* ident_dev = nullptr;        // [nb] identity index list
     int* wake_idx = nullptr; int wake_cap = 0;   // [wake_cap] device copy of the body indices of the last wake_impl call
+    std::vector<uint4> filters;      // [collider_cap] host copy of World::c_filter
     float* stage_host = nullptr;     // pinned host staging (2 * nb * 13 floats: in, out)
     cudaStream_t stream = nullptr;   // (the emulation has none)
 #if RB_DEVICE_BUILD
@@ -952,6 +953,10 @@ static int check_bodies(const RbWorld* W, int n, const int32_t* indices, const c
         if (indices[k] < 0 || indices[k] >= W->w.nb || (type >= 0 && W->bodies[indices[k]].body_type != type)) { set_err("%s", why); return RB_ERR_INVALID; }
     return RB_OK;
 }
+
+// World::c_filter of a collider that keeps the defaults: solver groups all() in And mode, ActiveCollisionTypes::default(),
+// collision groups in And mode.
+static const uint4 DEFAULT_FILTER = {0xffffffffu, 0xffffffffu, (unsigned)RB_ACT_DEFAULT, 0u};
 
 // Flags what the next step rebuilds: the broad-phase lists (1: movers, 3: static colliders too), the pair set, the islands and
 // the schedule.  A zero argument leaves that flag as it is.
@@ -1449,7 +1454,6 @@ int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t
     w.ev_cap = w.pair_cap;
     ALLOC(w.ev_coll, w.ev_cap); ALLOC(w.ev_force, (size_t)3 * w.ev_cap);
     for (int k = 0; k < 2; ++k) { ALLOC(w.pb[k].key, w.pair_cap); ALLOC(w.pb[k].rows, (size_t)PR_ROWS * w.pair_cap); }
-    ALLOC(w.todo, 16);
     ALLOC(w.color_mask, (size_t)NB * 4); ALLOC(w.body_min, NB); ALLOC(w.body_minkey, NB);
     ALLOC(w.isl_label, NB); ALLOC(w.isl_nb, NB); ALLOC(w.isl_ncons, NB); ALLOC(w.isl_item, NB);
     ALLOC(w.scan_tmp, (size_t)1 << 20);
@@ -1495,6 +1499,14 @@ int rb_world_set_scene(RbWorld* W, int32_t nb, const RbBodyDesc* bodies, int32_t
         CK(h2d(w.body_min, bmin.data(), NB * sizeof(int)));
         CK(dev_set(w.body_minkey, 0xff, NB * sizeof(unsigned long long)));
         CK(h2d(w.c_parent, parent.data(), NC * sizeof(int)));
+        {   // c_filter, preceded by the fixed-fixed pair keys (pair_cap is even: a whole number of uint4); allocated after the
+            // tables every world uses
+            uint4* block = nullptr;
+            ALLOC(block, (size_t)w.pair_cap / 2 + NC);
+            w.c_filter = block + w.pair_cap / 2;
+        }
+        W->filters.assign(NC, DEFAULT_FILTER);   // (every collider, inserted ones included, starts with the default filters)
+        CK(h2d(w.c_filter, W->filters.data(), (size_t)NC * sizeof(uint4)));
         rc = upload_bodies(W, mp, 0, nb);
         if (rc != RB_OK) return rc;
         rc = upload_hulls(W);
@@ -1759,6 +1771,75 @@ int rb_world_update_joints(RbWorld* W, int32_t n, const int32_t* indices, const 
     if ((rc = joints_changed(W)) != RB_OK) return rc;
     if (wake_up && !wake.empty()) return wake_impl(W, wake.data(), (int)wake.size());
     return RB_OK;
+}
+
+// Collider::set_collision_groups / set_solver_groups / set_active_collision_types.  The collision groups go to c_groups, the rest
+// to c_filter; the first collider given a filter that differs from the defaults switches the world to the filtered code paths
+// (World::has_filters) for the rest of the scene.  The next step re-runs the broad phase, which drops the pairs the new filters
+// forbid and finds the ones they allow (a changed static collider also re-runs the fixed-fixed search); the narrow phase
+// recomputes the pairs whose solver outcome changed.  As in the reference (narrow_phase/pair_management.rs:230-257), the
+// changed colliders' bodies and the bodies of every collider they share a pair with are woken: a fixed or kinematic parent
+// does not pass a wake-up on.
+int rb_world_set_collider_filters(RbWorld* W, int32_t n, const int32_t* indices, const RbColliderFilter* filters) {
+    if (!W || n < 0 || (n && (!indices || !filters)) || !W->w.st) { set_err("invalid arguments"); return RB_ERR_INVALID; }
+    const unsigned known = RB_ACT_DYNAMIC_DYNAMIC | RB_ACT_DYNAMIC_KINEMATIC | RB_ACT_DYNAMIC_FIXED | RB_ACT_KINEMATIC_KINEMATIC |
+                           RB_ACT_KINEMATIC_FIXED | RB_ACT_FIXED_FIXED;
+    for (int k = 0; k < n; ++k) {
+        const int c = indices[k];
+        const int p = c >= 0 && c < W->w.nc ? W->colliders[c].parent : -1;
+        if (c < 0 || c >= W->w.nc || (p >= 0 && W->bodies[p].body_type == BODY_REMOVED)) { set_err("collider index out of range (or removed)"); return RB_ERR_INVALID; }
+        const RbColliderFilter& f = filters[k];
+        if ((unsigned)f.collision_test_mode > 1u || (unsigned)f.solver_test_mode > 1u) { set_err("interaction test mode is neither RB_TEST_AND nor RB_TEST_OR"); return RB_ERR_INVALID; }
+        if (f.active_collision_types & ~known) { set_err("unknown active collision type bits"); return RB_ERR_INVALID; }
+    }
+    int rc = sync_world(W);
+    if (rc != RB_OK) return rc;
+    std::vector<unsigned char> changed(W->w.nc, 0);
+    int lo = W->w.nc, hi = -1, lists = 0;
+    for (int k = 0; k < n; ++k) {   // the host copies first, then one upload of the changed range
+        const int c = indices[k];
+        const RbColliderFilter& f = filters[k];
+        RbColliderDesc& d = W->colliders[c];
+        const uint4 extra = make_uint4(f.solver_memberships, f.solver_filter, f.active_collision_types,
+                                       (unsigned)f.collision_test_mode | ((unsigned)f.solver_test_mode << 1));
+        const uint4 old = W->filters[c];
+        if (d.collision_memberships == f.collision_memberships && d.collision_filter == f.collision_filter && old.x == extra.x &&
+            old.y == extra.y && old.z == extra.z && old.w == extra.w)
+            continue;
+        changed[c] = 1;
+        lo = std::min(lo, c);
+        hi = std::max(hi, c);
+        d.collision_memberships = f.collision_memberships;
+        d.collision_filter = f.collision_filter;
+        W->filters[c] = extra;
+        if (extra.x != DEFAULT_FILTER.x || extra.y != DEFAULT_FILTER.y || extra.z != DEFAULT_FILTER.z || extra.w != DEFAULT_FILTER.w)
+            W->w.has_filters = 1;
+        if (d.parent < 0 || !type_moves(W->bodies[d.parent].body_type)) lists = 3;   // (a static collider: re-run the fixed-fixed search)
+    }
+    if (hi < 0) return RB_OK;
+    {
+        std::vector<uint2> groups(hi - lo + 1);
+        for (int c = lo; c <= hi; ++c) groups[c - lo] = make_uint2(W->colliders[c].collision_memberships, W->colliders[c].collision_filter);
+        CK(h2d(W->w.c_groups + lo, groups.data(), groups.size() * sizeof(uint2)));
+        CK(h2d(W->w.c_filter + lo, W->filters.data() + lo, (size_t)(hi - lo + 1) * sizeof(uint4)));
+    }
+    std::vector<int32_t> wake;
+    for (int c = lo; c <= hi; ++c)
+        if (changed[c] && W->colliders[c].parent >= 0) wake.push_back(W->colliders[c].parent);
+    State st;
+    CK(d2h(&st, W->w.st, sizeof(State)));
+    if (st.npairs > 0) {
+        std::vector<unsigned long long> keys(st.npairs);
+        CK(d2h(keys.data(), W->w.pb[st.cur].key, (size_t)st.npairs * 8));
+        for (unsigned long long key : keys) {
+            const int c1 = (int)(key >> 32), c2 = (int)(key & 0xffffffffu);
+            if (!changed[c1] && !changed[c2]) continue;
+            if (W->colliders[c1].parent >= 0) wake.push_back(W->colliders[c1].parent);
+            if (W->colliders[c2].parent >= 0) wake.push_back(W->colliders[c2].parent);
+        }
+    }
+    if ((rc = mark_dirty(W, lists, 1, 0)) != RB_OK) return rc;
+    return wake.empty() ? RB_OK : wake_impl(W, wake.data(), (int)wake.size());
 }
 
 int rb_world_set_body_states(RbWorld* W, int32_t n, const int32_t* indices, const float* pose7, const float* vel6) {

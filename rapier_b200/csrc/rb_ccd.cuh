@@ -148,6 +148,15 @@ RB_HD bool ccd_is_moving_fast(const Params& P, vec3 lcom, const pose& op, const 
     return max2(max_delta_position, max_velocity * P.dt) > 0.5f * thickness;
 }
 
+// Whether collider c's sweep may stop at collider cj: their collision groups pass and, in a world with collider filters, in
+// their test modes, and so do their solver groups -- a pair without forces is a pseudo-hit the sweep ignores (sweeps.rs:563-568).
+RB_HD bool ccd_groups_allow(const World& w, int c, int cj, uint2 g1) {
+    const uint2 g2 = w.c_groups[cj];
+    if (!w.has_filters) return (g1.x & g2.y) != 0 && (g2.x & g1.y) != 0;
+    const uint4 f1 = w.c_filter[c], f2 = w.c_filter[cj];
+    return groups_test(g1.x, g1.y, f1.w & 1u, g2.x, g2.y, f2.w & 1u) && groups_test(f1.x, f1.y, f1.w >> 1, f2.x, f2.y, f2.w >> 1);
+}
+
 // sweep_fast_body + apply_clamps for one fast, non-bullet body: the earliest impact of any of its colliders against
 // the fixed colliders, and the pose at that fraction of the body's own sweep.  One thread; fast bodies are rare.
 // (Always inlined: as an out-of-line call inside k_collide -- ABI call, 900 B more stack -- it costs time on every step of the
@@ -180,8 +189,7 @@ RB_HD pose ccd_clamp_body(const World& w, int b, pose op, pose np, bool bullet =
             if (pj >= 0 && w.b_type[pj] != BODY_FIXED) return;   // tier_allows (sweeps.rs:36-42): non-bullets only hit fixed targets
             if (w.c_shape[cj] >= SHAPE_CAPSULE) return;
             if (w.has_sensors && (w.c_events[cj] & 4)) return;
-            const uint2 g2 = w.c_groups[cj];
-            if (!((g1.x & g2.y) != 0 && (g2.x & g1.y) != 0)) return;
+            if (!ccd_groups_allow(w, c, cj, g1)) return;
             const float f = ccd_toi(w.c_shape[cj], xyz(w.c_he[cj]), collider_pose(w, cj), sh, he, sw, slop);
             if (f > 0.0f && f < frac) frac = f;
         };
@@ -198,8 +206,7 @@ RB_HD pose ccd_clamp_body(const World& w, int b, pose op, pose np, bool bullet =
                 if (w.has_sensors && (w.c_events[cj] & 4)) continue;
                 if (w.b_type[pj] == BODY_DYNAMIC && (w.b_flags[pj] & FLAG_CCD)) continue;
                 if (!fat_overlap(amin, amax, w.c_fat_min[cj], w.c_fat_max[cj])) continue;
-                const uint2 g2 = w.c_groups[cj];
-                if (!((g1.x & g2.y) != 0 && (g2.x & g1.y) != 0)) continue;
+                if (!ccd_groups_allow(w, c, cj, g1)) continue;
                 const pose tp = pmul(body_pose(w, pj), mkpose(mkq(w.c_rel_q[cj]), xyz(w.c_rel_t[cj])));
                 const float f = ccd_toi(shj, xyz(w.c_he[cj]), tp, sh, he, sw, slop);
                 if (f > 0.0f && f < frac) frac = f;

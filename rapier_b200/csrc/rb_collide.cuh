@@ -236,14 +236,48 @@ RB_PHASE unsigned long long* grid_radix_sort(const Ctx& ctx, unsigned long long*
     return a;
 }
 
+// InteractionGroups::test (interaction_groups.rs:136-154): Or applies only when both sides use it, And takes priority.
+RB_HD bool groups_test(unsigned m1, unsigned f1, unsigned or1, unsigned m2, unsigned f2, unsigned or2) {
+    const bool a = (m1 & f2) != 0, b = (m2 & f1) != 0;
+    return (or1 & or2) ? (a || b) : (a && b);
+}
+// ActiveCollisionTypes::test (collider_components.rs:300-334) on body types numbered like RigidBodyType.
+RB_HD bool collision_types_test(unsigned bits, int t1, int t2) {
+    return (((bits >> (t1 * 4)) & 15u) & (1u << t2)) != 0 || (((bits >> (t2 * 4)) & 15u) & (1u << t1)) != 0;
+}
+RB_HD int filter_body_type(const World& w, int b) { return b < 0 ? BODY_FIXED : w.b_type[b]; }   // (a parentless collider is fixed)
+// The solver groups fail, or neither body is dynamic: the pair keeps its contacts and touch events but computes no force
+// (SolverFlags without COMPUTE_IMPULSES, pair_update.rs:279-281).  Worlds with collider filters only.
+RB_HD bool pair_forceless(const World& w, int c1, int c2, int b1, int b2) {
+    if (filter_body_type(w, b1) != BODY_DYNAMIC && filter_body_type(w, b2) != BODY_DYNAMIC) return true;
+    const uint4 f1 = w.c_filter[c1], f2 = w.c_filter[c2];
+    return !groups_test(f1.x, f1.y, f1.w >> 1, f2.x, f2.y, f2.w >> 1);
+}
+
 // update.rs:334-396 filter_new
 RB_HD bool pair_allowed(const World& w, int c1, int c2) {
     int p1 = w.c_parent[c1], p2 = w.c_parent[c2];
     if (p1 >= 0 && p1 == p2) return false;
     bool d1 = body_is_strict_dyn(w, p1), d2 = body_is_strict_dyn(w, p2);   // (sleeping bodies keep their pairs)
-    if (!d1 && !d2) return false;   // ActiveCollisionTypes::default(): DYNAMIC_DYNAMIC | DYNAMIC_KINEMATIC | DYNAMIC_FIXED
     uint2 g1 = w.c_groups[c1], g2 = w.c_groups[c2];
-    if (!((g1.x & g2.y) != 0 && (g2.x & g1.y) != 0)) return false;
+    if (w.has_filters) {   // (a kernel parameter: uniform)
+        // the collision types of either collider (update.rs:361-385; solver groups are not tested here, :365-366), then the
+        // mode-aware collision groups.  Which rank keeps the pair (multi-GPU sharding): a pair with a dynamic body simulated
+        // here is kept as without filters; a pair whose only dynamic bodies belong to other ranks is not; a pair without a
+        // dynamic body is kept by the rank that simulates its lower-indexed body (every rank, for two parentless colliders).
+        const int t1 = filter_body_type(w, p1), t2 = filter_body_type(w, p2);
+        if (!d1 && !d2) {
+            if (t1 == BODY_DYNAMIC || t2 == BODY_DYNAMIC) return false;
+            const int lo = p1 < 0 ? p2 : (p2 < 0 ? p1 : (p1 < p2 ? p1 : p2));
+            if (lo >= 0 && w.b_owned[lo] != 1) return false;
+        }
+        const uint4 f1 = w.c_filter[c1], f2 = w.c_filter[c2];
+        if (!collision_types_test(f1.z, t1, t2) && !collision_types_test(f2.z, t1, t2)) return false;
+        if (!groups_test(g1.x, g1.y, f1.w & 1u, g2.x, g2.y, f2.w & 1u)) return false;
+    } else {
+        if (!d1 && !d2) return false;   // ActiveCollisionTypes::default(): DYNAMIC_DYNAMIC | DYNAMIC_KINEMATIC | DYNAMIC_FIXED
+        if (!((g1.x & g2.y) != 0 && (g2.x & g1.y) != 0)) return false;
+    }
     if (w.n_nocontact > 0 && p1 >= 0 && p2 >= 0) {
         unsigned lo = (unsigned)(p1 < p2 ? p1 : p2), hi = (unsigned)(p1 < p2 ? p2 : p1);
         if (bsearch_u64(w.nocontact_keys, w.n_nocontact, ((unsigned long long)lo << 32) | hi) >= 0) return false;
@@ -283,6 +317,40 @@ RB_HD void emit_candidate(const World& w, int ci, int cj) {
 
 constexpr int WIDE_CAP = 1024;   // static colliders much wider than the rest (a ground slab under a tiled floor): tested by every mover
 
+// Fixed-fixed pairs (ActiveCollisionTypes::FIXED_FIXED, broad_phase_bvh/update.rs:361-385): the sweep below starts from the
+// movers only, so two static colliders never meet there.  When the static lists are rebuilt, every static collider that opts in
+// is searched, one thread each, against the sorted static keys and the wide list; the pairs found stay in ff_keys and join
+// every later candidate set (section_broad_phase).
+constexpr unsigned ACT_FIXED_FIXED = 0x0020u;
+template <class Ctx>
+RB_PHASE void section_fixed_pairs(const Ctx& ctx, const World& w, const unsigned long long* skey) {
+    State* st = w.st;
+    const int ns = st->nstat, nwide = st->nwide < WIDE_CAP ? st->nwide : WIDE_CAP;
+    const float wn = as_float(st->stat_wn_bits) * 1.0001f + 1.0e-6f;   // widest narrow static collider (with rounding slack)
+    unsigned long long* ff = ff_keys(w);
+    for (int c = ctx.gtid; c < w.nc; c += ctx.gsize) {
+        if (w.c_shape[c] == SHAPE_REMOVED || !collider_is_static(w, c) || !(w.c_filter[c].z & ACT_FIXED_FIXED)) continue;
+        const float4 amin = w.c_fat_min[c], amax = w.c_fat_max[c];
+        auto test = [&](int j) {
+            if (j == c || (j < c && (w.c_filter[j].z & ACT_FIXED_FIXED))) return;   // (two opted-in colliders: found from the lower one)
+            if (!fat_overlap(amin, amax, w.c_fat_min[j], w.c_fat_max[j])) return;
+            const int c1 = c < j ? c : j, c2 = c < j ? j : c;
+            if (!pair_allowed(w, c1, c2)) return;
+            const int slot = atomic_add(&st->nff, 1);
+            if (slot < w.pair_cap) ff[slot] = ((unsigned long long)(unsigned)c1 << 32) | (unsigned)c2;
+        };
+        const unsigned amax_key = sortable_float(amax.x);
+        for (int j = lower_bound_u64(skey, ns, (unsigned long long)sortable_float(amin.x - wn) << 32); j < ns; ++j) {
+            const unsigned long long kj = skey[j];
+            if ((unsigned)(kj >> 32) > amax_key) break;
+            test((int)(kj & 0xffffffffu));
+        }
+        for (int k = 0; k < nwide; ++k) test(w.wide_list[k]);
+    }
+    ctx.grid_sync();
+    if (ctx.gtid == 0 && st->nff > w.pair_cap) RB_RAISE(w, -4);   // (the list keeps what fits; the status reports the rest)
+}
+
 // P1 (lists): split the colliders into the movers (sorted every time an AABB changes) and the static ones (sorted
 // here, once): the reference keeps all leaves in one tree and only re-tests CHANGED leaves (broad_phase_bvh/
 // update.rs:441-601), which static leaves never are.  Static colliders much wider along x than the average go to a
@@ -293,7 +361,7 @@ RB_PHASE void section_build_lists(const Ctx& ctx, const World& w) {
     const bool statics = (st->lists_dirty & 2) != 0;   // bit 1: the static colliders changed too (else only movers were added)
     if (ctx.gtid == 0) {
         st->ndyn = 0;
-        if (statics) { st->nstat = 0; st->nwide = 0; st->stat_count = 0; st->stat_wsum = 0.0f; st->stat_wn_bits = 0u; }
+        if (statics) { st->nstat = 0; st->nwide = 0; st->stat_count = 0; st->stat_wsum = 0.0f; st->stat_wn_bits = 0u; st->nff = 0; }
     }
     if (statics) grid_radix_zero(ctx, w.radix_hist, 4);
     ctx.grid_sync();
@@ -329,6 +397,7 @@ RB_PHASE void section_build_lists(const Ctx& ctx, const World& w) {
     if (statics) {
         unsigned long long* sorted = grid_radix_sort(ctx, w.stat_key[0], w.stat_key[1], st->nstat, 32, 64, w.radix_hist);
         if (ctx.gtid == 0) st->stat_sorted = sorted == w.stat_key[0] ? 0 : 1;
+        if (w.has_filters) section_fixed_pairs(ctx, w, sorted);   // (a kernel parameter: uniform)
     }
     if (ctx.gtid == 0) { st->lists_dirty = 0; st->bp_dirty = 1; }
     ctx.grid_sync();
@@ -431,6 +500,11 @@ RB_PHASE void section_broad_phase(const Ctx& ctx, const World& w) {
             const int cj = w.wide_list[k];
             if (fat_overlap(amin, amax, w.c_fat_min[cj], w.c_fat_max[cj])) emit_candidate(w, ci, cj);
         }
+    }
+    if (w.has_filters) {   // the fixed-fixed pairs of the last static rebuild (section_fixed_pairs), filtered again
+        const int nff = st->nff < w.pair_cap ? st->nff : w.pair_cap;
+        const unsigned long long* ff = ff_keys(w);
+        for (int k = ctx.gtid; k < nff; k += ctx.gsize) emit_candidate(w, (int)(ff[k] >> 32), (int)(ff[k] & 0xffffffffu));
     }
     const int cbits = bits_for(w.nc > 2 ? w.nc : 2);
     const int p_lo = radix_passes(0, cbits), p_hi = radix_passes(32, 32 + cbits);
@@ -583,8 +657,8 @@ RB_PHASE void phase_convex_manifolds(const Ctx& ctx, const World& w) {
         const int c1 = (int)(key >> 32), c2 = (int)(key & 0xffffffffu);
         if (!pair_is_poly_poly(w.c_shape[c1], w.c_shape[c2])) continue;
         const float4 bod0 = prow(w, buf, PR_BODIES, i);
-        if (!body_is_sim(w, as_int(bod0.z)) && !body_is_sim(w, as_int(bod0.w))) continue;
         const int flags = as_int(prow(w, buf, PR_INFO, i).x);
+        if (!body_is_sim(w, as_int(bod0.z)) && !body_is_sim(w, as_int(bod0.w)) && !(w.has_filters && !(flags & 64))) continue;
         if (recycle > 0.0f && (flags & 1)) {
             const pose cp1 = collider_pose(w, c1), cp2 = collider_pose(w, c2);
             const pose p12 = pinv_mul(cp1, cp2);
@@ -634,15 +708,24 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
         int c1 = (int)(key >> 32), c2 = (int)(key & 0xffffffffu);
         {   // pairs without an AWAKE body simulated by this rank are not updated: they belong to another rank
             // (multi-GPU sharding) or to a sleeping island, whose bodies do not move
+            // (with collider filters, a pair the narrow phase has never updated is updated once whatever its bodies: a pair of two
+            // static colliders, or a pair that a filter change brought back under a sleeping body)
             float4 bod0 = prow(w, buf, PR_BODIES, i);
-            if (!body_is_sim(w, as_int(bod0.z)) && !body_is_sim(w, as_int(bod0.w))) continue;
+            if (!body_is_sim(w, as_int(bod0.z)) && !body_is_sim(w, as_int(bod0.w)) &&
+                !(w.has_filters && !(as_int(prow(w, buf, PR_INFO, i).x) & 64)))
+                continue;
         }
         pose cp1 = collider_pose(w, c1), cp2 = collider_pose(w, c2);
         float4 info = prow(w, buf, PR_INFO, i);
         int flags = as_int(info.x), npts_old = as_int(info.y), nsc_old = as_int(info.z), color = as_int(info.w);
         pose p12 = pinv_mul(cp1, cp2);
-        // contact recycling (pair_update.rs:111-171)
-        if (recycle > 0.0f && (flags & 1)) {
+        bool forceless = false;
+        if (w.has_filters) {   // (a kernel parameter: uniform)
+            const float4 bodf = prow(w, buf, PR_BODIES, i);
+            forceless = pair_forceless(w, c1, c2, as_int(bodf.z), as_int(bodf.w));
+        }
+        // contact recycling (pair_update.rs:111-171); a pair whose solver outcome changed is recomputed (:116-121)
+        if (recycle > 0.0f && (flags & 1) && forceless == ((flags & 32) != 0)) {
             float4 rt = prow(w, buf, PR_RT, i);
             pose base = mkpose(mkq(prow(w, buf, PR_RQ, i)), xyz(rt));
             float drift = pose_drift(base, p12, rt.w);
@@ -666,7 +749,7 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
             bool inter = false;
             for (int k = 0; k < raw.n; ++k) inter = inter || raw.pt[k].dist <= 0.0f;
             if (inter != ((flags & 16) != 0)) emit_collision_event(w, c1, c2, inter);
-            prow(w, buf, PR_INFO, i) = make_float4(as_float_i(inter ? 16 : 0), as_float_i(0), as_float_i(0), as_float_i(color));
+            prow(w, buf, PR_INFO, i) = make_float4(as_float_i((inter ? 16 : 0) | (w.has_filters ? 64 : 0)), as_float_i(0), as_float_i(0), as_float_i(color));
             continue;
         }
 
@@ -729,6 +812,7 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
                     pd = o_pd[o]; tw = o_tw[o]; d1 = o_d1[o]; d2 = o_d2[o];
                 }
             }
+            if (forceless) { pd = make_float4(0.f, 0.f, 0.f, 0.f); tw = pd; }   // (no impulse, nothing to warm-start)
             pd.w = as_float(rp.fid2);
             float eff = rp.dist - skin1 - skin2;
             vec3 wp1 = xform(cp1, rp.p1), wp2 = xform(cp2, rp.p2);
@@ -781,8 +865,10 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
             emit_collision_event(w, c1, c2, has);
             if (!has) flags &= ~8;   // the force-event status resets when the colliders separate (geometry/mod.rs:208-217)
             if (has) {
-                flags |= 2;  // pending colour (deferred greedy pass)
-                st->ntodo = 1;
+                if (!forceless) {
+                    flags |= 2;  // pending colour (deferred greedy pass)
+                    st->ntodo = 1;
+                }
                 // a contact that begins wakes the sleeping side's whole island (narrow_phase/mod.rs:53-67)
                 if (dyn1 && w.b_sleeping[b1]) { w.wake_req[w.isl_label[b1]] = 1; st->wake_any = 1; }
                 if (dyn2 && w.b_sleeping[b2]) { w.wake_req[w.isl_label[b2]] = 1; st->wake_any = 1; }
@@ -791,6 +877,21 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
                 color = COLOR_UNCOLORED;
                 prow(w, buf, PR_BODIES, i) = make_float4(as_float_i(-1), as_float_i(-1), bod.z, bod.w);
             }
+        }
+        if (w.has_filters) {
+            if (had && has && forceless != ((flags & 32) != 0)) {   // a touching pair gains or loses its forces: recolour, reschedule
+                st->sched_dirty = 1;
+                if (forceless) {
+                    clear_color_bits(w, color, as_int(bod.x), as_int(bod.y));
+                    color = COLOR_UNCOLORED;
+                    flags &= ~8;
+                    prow(w, buf, PR_BODIES, i) = make_float4(as_float_i(-1), as_float_i(-1), bod.z, bod.w);
+                } else {
+                    flags |= 2;
+                    st->ntodo = 1;
+                }
+            }
+            flags = (forceless ? (flags | 32) : (flags & ~32)) | 64;
         }
         prow(w, buf, PR_INFO, i) = make_float4(as_float_i(flags), as_float_i(nsel), as_float_i(nsc), as_float_i(color));
     }
@@ -1019,7 +1120,10 @@ RB_PHASE void section_components(const Ctx& ctx, const World& w) {
         if (as_int(prow(w, buf, PR_INFO, i).z) <= 0) continue;
         float4 bod = prow(w, buf, PR_BODIES, i);
         int b1 = as_int(bod.z), b2 = as_int(bod.w);
-        if (body_is_dyn(w, b1) && body_is_dyn(w, b2)) uf_union(w.isl_label, b1, b2);
+        // Two touching kinematic bodies are no island edge.  A touching pair whose solver groups fail still is one, as the
+        // reference links islands over every pair with an active contact whatever its solver flags (substep_groups.rs:73-87).
+        if (body_is_dyn(w, b1) && body_is_dyn(w, b2) && !(w.has_filters && w.b_type[b1] != BODY_DYNAMIC && w.b_type[b2] != BODY_DYNAMIC))
+            uf_union(w.isl_label, b1, b2);
     }
     for (int j = ctx.gtid; j < nj; j += ctx.gsize) {
         int4 ji = w.j_info[j];
@@ -1119,7 +1223,7 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         }
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
         float4 info = prow(w, buf, PR_INFO, i);
-        if (as_int(info.z) <= 0) continue;
+        if (as_int(info.z) <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;   // (forceless pairs are no constraint)
         float4 bod = prow(w, buf, PR_BODIES, i);
         int b1 = as_int(bod.z), b2 = as_int(bod.w);
         int b = body_is_sim(w, b1) ? b1 : (body_is_sim(w, b2) ? b2 : -1);
@@ -1201,7 +1305,8 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         if (w.any_extra) w.b_key[b] = (unsigned char)(it >= 0 ? w.isl_key[w.isl_label[b]] : 0u);
     }
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
-        if (as_int(prow(w, buf, PR_INFO, i).z) <= 0) continue;
+        const float4 info = prow(w, buf, PR_INFO, i);
+        if (as_int(info.z) <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;
         float4 bod = prow(w, buf, PR_BODIES, i);
         int b1 = as_int(bod.z), b2 = as_int(bod.w);
         int b = body_is_sim(w, b1) ? b1 : (body_is_sim(w, b2) ? b2 : -1);
@@ -1235,7 +1340,8 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         w.body_local[b] = l;
     }
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
-        if (as_int(prow(w, buf, PR_INFO, i).z) <= 0) continue;
+        const float4 info = prow(w, buf, PR_INFO, i);
+        if (as_int(info.z) <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;
         float4 bod = prow(w, buf, PR_BODIES, i);
         int b1 = as_int(bod.z), b2 = as_int(bod.w);
         int b = body_is_sim(w, b1) ? b1 : (body_is_sim(w, b2) ? b2 : -1);

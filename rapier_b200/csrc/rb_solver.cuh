@@ -1171,7 +1171,7 @@ RB_PHASE void phase_force_events(const Ctx& ctx, const World& w) {
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
         float4 info = prow(w, buf, PR_INFO, i);
         const int nsc = as_int(info.z);
-        if (nsc <= 0) continue;
+        if (nsc <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;   // (a pair without forces raises no force event)
         const unsigned long long key = w.pb[buf].key[i];
         const int c1 = (int)(key >> 32), c2 = (int)(key & 0xffffffffu);
         const float t1 = (w.c_events[c1] & 2) ? w.c_force_thr[c1] : FMAX32, t2 = (w.c_events[c2] & 2) ? w.c_force_thr[c2] : FMAX32;

@@ -44,7 +44,9 @@ struct HullTables {
 
 // ---- persistent pair record rows (float4 each) ----
 enum PairRow {
-    PR_INFO = 0,   // int bits: x flags(bit0 has_recycle, bit1 pending colour, bit2 colouring scratch, bit3 force event emitted last step, bit4 sensor pair intersecting), y npts, z nsc, w colour
+    PR_INFO = 0,   // int bits: x flags(bit0 has_recycle, bit1 pending colour, bit2 colouring scratch, bit3 force event emitted last step, bit4 sensor pair intersecting,
+                   //   worlds with collider filters only: bit5 contacts without forces (solver groups fail or no dynamic body),
+                   //   bit6 the narrow phase has updated the pair at least once), y npts, z nsc, w colour
     PR_BODIES,     // int bits: x colour_body0, y colour_body1, z body1, w body2 (-1 none)
     PR_RT,         // recycle pos12.t xyz, w max_extent
     PR_RQ,         // recycle pos12.q
@@ -140,6 +142,7 @@ struct State {
     int nccd_bullets;      // ... of which bullets (ccd_enabled): they sweep in a second pass, against the already clamped poses
     int nev_coll, nev_force;   // buffered collision / contact-force events since the host last drained them
     int nconvex;           // polyhedron pairs whose manifold the warps compute together this step (World::convex_work)
+    int nff;               // fixed-fixed pairs found when the static lists were last rebuilt (ff_keys; worlds with collider filters)
 };
 
 struct PairBuf {
@@ -195,6 +198,7 @@ struct World {
     uint2* c_groups;
     int* c_events;                    // ActiveEvents bits (1 = collision events, 2 = contact force events) | 4 = the collider is a sensor
     int has_sensors;                  // some collider is a sensor (Collider::is_sensor): intersection-only pairs exist
+    int has_filters;                  // some collider holds filters other than the defaults (c_filter); no other world reads c_filter
     float* c_force_thr;               // contact_force_event_threshold
     float4 *c_pos_t, *c_pos_q;
     float4 *c_aabb_min, *c_aabb_max, *c_fat_min, *c_fat_max;
@@ -217,7 +221,10 @@ struct World {
     int step_index;                   // index of the step being enqueued (1 = first step after the scene upload)
     // ---- pairs ----
     PairBuf pb[2];
-    int* todo;                        // [pair_cap] pairs that began touching this step
+    // Collider filters beyond the collision groups (ColliderFlags, collider_components.rs:363-379; rb_world_set_collider_filters).
+    // (Placed here, and has_filters in the padding after has_sensors, so that World keeps its layout for the kernels.)
+    // The same allocation holds, just below c_filter, the [pair_cap] keys of the fixed-fixed pairs (ff_keys, State::nff).
+    uint4* c_filter;                  // [nc] solver memberships, solver filter, ActiveCollisionTypes bits, collision test mode | solver test mode << 1
     unsigned* color_mask;             // [nb][4] 128-bit colour masks per body
     int* body_min;                    // [nb] colouring scratch (INT_MAX when idle)
     unsigned long long* body_minkey;  // [nb] colouring scratch: smallest pending order key (~0 when idle)
@@ -300,6 +307,7 @@ enum JointRowRec {
     JR_ROWS
 };
 
+RB_HD unsigned long long* ff_keys(const World& w) { return reinterpret_cast<unsigned long long*>(w.c_filter) - w.pair_cap; }
 RB_HD float4& prow(const World& w, int buf, int row, int i) { return w.pb[buf].rows[(size_t)row * w.pair_cap + i]; }
 RB_HD float4& crow(const World& w, int row, int i) { return w.cons[(size_t)row * w.cons_cap + i]; }
 RB_HD float4& jrow(const World& w, int row, int i) { return w.j_rows[(size_t)row * (6 * w.joint_cap) + i]; }

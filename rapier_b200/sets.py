@@ -266,10 +266,32 @@ class ColliderBuilder:
         self._contact_skin = float(s)
         return self
 
-    def collision_groups(self, memberships, filter_):
+    def collision_groups(self, memberships, filter_, test_mode=A.RB_TEST_AND):
+        """ColliderBuilder::collision_groups (InteractionGroups; test_mode: RB_TEST_AND or RB_TEST_OR)."""
         self._memberships = int(memberships)
         self._filter = int(filter_)
+        self._collision_test_mode = int(test_mode)
         return self
+
+    def solver_groups(self, memberships, filter_, test_mode=A.RB_TEST_AND):
+        """ColliderBuilder::solver_groups: a pair whose solver groups fail keeps its contacts and events but gets no force."""
+        self._solver_groups = (int(memberships), int(filter_), int(test_mode))
+        return self
+
+    def active_collision_types(self, bits):
+        """ColliderBuilder::active_collision_types (RB_ACT_* bits; default RB_ACT_DEFAULT)."""
+        self._active_collision_types = int(bits)
+        return self
+
+    def build_filter(self):
+        """The collider's RbColliderFilter, or None when everything but the collision groups (which travel in the
+        descriptor) keeps its default."""
+        mode = getattr(self, "_collision_test_mode", A.RB_TEST_AND)
+        solver = getattr(self, "_solver_groups", (0xFFFFFFFF, 0xFFFFFFFF, A.RB_TEST_AND))
+        types = getattr(self, "_active_collision_types", A.RB_ACT_DEFAULT)
+        if mode == A.RB_TEST_AND and solver == (0xFFFFFFFF, 0xFFFFFFFF, A.RB_TEST_AND) and types == A.RB_ACT_DEFAULT:
+            return None
+        return A.RbColliderFilter(self._memberships, self._filter, mode, *solver, types)
 
     def active_events(self, events):
         """ColliderBuilder::active_events (ActiveEvents: RB_EVENT_COLLISION | RB_EVENT_CONTACT_FORCE)."""
@@ -469,6 +491,7 @@ class RigidBodySet:
 class ColliderSet:
     def __init__(self):
         self.descs = []
+        self.filters = {}      # collider index -> RbColliderFilter, for the colliders whose filters are not the defaults
         self.hulls = []        # convex polyhedra referred to by RB_SHAPE_CONVEX colliders: (vertices [n, 3] f32, faces); id = index + 1
         self._hull_ids = {}
 
@@ -484,12 +507,23 @@ class ColliderSet:
         return d
 
     def insert(self, builder):
-        self.descs.append(self._desc(builder, None))
-        return len(self.descs) - 1
+        return self.insert_with_parent(builder, None)
 
     def insert_with_parent(self, builder, parent, bodies=None):
         self.descs.append(self._desc(builder, parent))
+        f = builder.build_filter()
+        if f is not None:
+            self.filters[len(self.descs) - 1] = f
         return len(self.descs) - 1
+
+    def filter(self, i):
+        """The current RbColliderFilter of collider i."""
+        f = self.filters.get(i)
+        if f is not None:
+            return A.RbColliderFilter.from_buffer_copy(f)
+        d = self.descs[i]
+        return A.RbColliderFilter(d.collision_memberships, d.collision_filter, A.RB_TEST_AND, 0xFFFFFFFF, 0xFFFFFFFF, A.RB_TEST_AND,
+                                  A.RB_ACT_DEFAULT)
 
     def __len__(self):
         return len(self.descs)

@@ -104,6 +104,13 @@ class PhysicsPipeline:
         j = as_array(joint_descs, A.RbJointDesc)
         self._check(self.L.rb_world_update_joints(self.h, len(idx), idx.ctypes.data, j, 1 if wake_up else 0))
 
+    def set_collider_filters(self, indices, filters):
+        """Collider::set_collision_groups / set_solver_groups / set_active_collision_types: collider indices[k] takes filters[k]
+        (RbColliderFilter) from the next step on."""
+        idx = np.ascontiguousarray(indices, np.int32)
+        f = as_array(filters, A.RbColliderFilter)
+        self._check(self.L.rb_world_set_collider_filters(self.h, len(idx), idx.ctypes.data, f))
+
     def set_params(self, params):
         self.params = params
         self._check(self.L.rb_world_set_params(self.h, C.byref(params)))
@@ -323,6 +330,11 @@ class PhysicsWorld:
                 self.physics_pipeline.insert(self.bodies.descs[nb0:], self.colliders.descs[nc0:])
             else:
                 self.physics_pipeline.upload(self.bodies, self.colliders, self.impulse_joints)
+                nc0 = 0
+            # the colliders just uploaded whose filters are not the defaults (a scene without any makes no such call)
+            new = sorted(i for i in self.colliders.filters if i >= nc0)
+            if new:
+                self.physics_pipeline.set_collider_filters(new, [self.colliders.filters[i] for i in new])
             self._uploaded = (nb, nc, nj)
             self._dirty = False
 
@@ -358,6 +370,30 @@ class PhysicsWorld:
         """RigidBody::set_position / set_linvel / set_angvel (wakes the bodies' islands)."""
         self._flush()
         self.physics_pipeline.set_body_states(handles, pose7, vel6)
+
+    def set_collider_filters(self, handles, collision_groups=None, solver_groups=None, active_collision_types=None):
+        """Collider::set_collision_groups / set_solver_groups / set_active_collision_types on the listed colliders, effective
+        from the next step.  collision_groups and solver_groups are (memberships, filter) or (memberships, filter, test_mode);
+        an argument left at None keeps the collider's current value."""
+        self._flush()
+        handles = [int(h) for h in handles]
+        new = []
+        for h in handles:
+            f = self.colliders.filter(h)
+            if collision_groups is not None:
+                g = tuple(collision_groups) + (A.RB_TEST_AND,) * (3 - len(collision_groups))
+                f.collision_memberships, f.collision_filter, f.collision_test_mode = g
+            if solver_groups is not None:
+                g = tuple(solver_groups) + (A.RB_TEST_AND,) * (3 - len(solver_groups))
+                f.solver_memberships, f.solver_filter, f.solver_test_mode = g
+            if active_collision_types is not None:
+                f.active_collision_types = int(active_collision_types)
+            new.append(f)
+        self.physics_pipeline.set_collider_filters(handles, new)
+        for h, f in zip(handles, new):   # (the sets mirror what the device now holds)
+            self.colliders.descs[h].collision_memberships = f.collision_memberships
+            self.colliders.descs[h].collision_filter = f.collision_filter
+            self.colliders.filters[h] = f
 
     def set_body_forces(self, handles, force3=None, torque3=None):
         self._flush()
