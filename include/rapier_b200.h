@@ -28,6 +28,10 @@ extern "C" {
 
 #define RB_ABI_VERSION 6
 
+/* Skin of the broad phase's fat boxes, in units of length_unit (BroadPhaseBvh::CHANGE_DETECTION_FACTOR): a collider's
+ * fat box is its tight box widened by this much, and is refitted only when the tight box leaves it. */
+#define RB_FAT_SKIN_FACTOR 4.0e-2f
+
 typedef struct RbWorld RbWorld;
 
 typedef enum RbStatus {

@@ -25,6 +25,7 @@ RB_BODY_NO_SLEEP = 256
 RB_BODY_CCD_ENABLED = 512
 RB_BODY_DOMINANCE_SHIFT = 16   # RB_BODY_DOMINANCE(group): signed 8-bit dominance group in bits 16..23 of flags
 RB_BODY_EXTRA_ITERS_SHIFT = 24  # RB_BODY_EXTRA_ITERS(n): additional_solver_iterations (0..255) in bits 24..31 of flags
+RB_FAT_SKIN_FACTOR = 0.04     # RB_FAT_SKIN_FACTOR: fat-box skin in units of length_unit
 RB_SHAPE_BALL = 0
 RB_SHAPE_CUBOID = 1
 RB_SHAPE_CAPSULE = 2

@@ -596,7 +596,7 @@ static void derive_params(const RbIntegrationParameters& p_in, Params& o, int ex
     o.prediction = p.normalized_prediction_distance * p.length_unit;
     o.recycle_dist = p.normalized_contact_recycle_distance * p.length_unit;
     o.length_unit = p.length_unit;
-    o.fat_skin = 4.0e-2f * p.length_unit;   // BroadPhaseBvh::CHANGE_DETECTION_FACTOR (broad_phase_bvh/mod.rs:175)
+    o.fat_skin = RB_FAT_SKIN_FACTOR * p.length_unit;   // BroadPhaseBvh::CHANGE_DETECTION_FACTOR (broad_phase_bvh/mod.rs:175)
     o.max_lin_vel = p.normalized_max_linear_velocity * p.length_unit;
     o.max_ang_vel = 0.7853981633974483f * o.inv_dt_full;   // MAX_ROTATION * inv_dt (worker.rs:573-580)
     o.num_pgs = p.num_internal_pgs_iterations;
@@ -2321,12 +2321,15 @@ int rb_debug_kat(const char* name, const float* in, int32_t n_in, float* out, in
 // ---- multi-GPU sharding ----
 int rb_world_label_components(RbWorld* W, int32_t* component_of_body) {
     if (!W || !component_of_body) return RB_ERR_INVALID;
-    // Run the collision pipeline once (it leaves poses untouched) so the island labels are current.
+    // Run the collision pipeline once (it leaves poses untouched) so the island labels are current.  Without the sleep
+    // decision: it advances every body's sleep timer by one step, and a query must not change what the next step computes.
     CK(set_device(W->device));
     CK(stream_sync(W->stream));
     int rc = mark_dirty(W, 0, 0, 1);
     if (rc != RB_OK) return rc;
-    CK(launch(W, W->ext_shapes ? k_collide<1> : k_collide<0>, W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, true, W->w, Grav{0.f, 0.f, 0.f}, 0));
+    World query = W->w;
+    query.sleep_enabled = 0;
+    CK(launch(W, W->ext_shapes ? k_collide<1> : k_collide<0>, W->collide_blocks, COLLIDE_THREADS, ITEM_SMEM_BYTES, true, query, Grav{0.f, 0.f, 0.f}, 0));
     if ((rc = sync_world(W)) != RB_OK) return rc;
     CK(d2h(component_of_body, W->w.isl_label, (size_t)W->w.nb * sizeof(int)));
     for (int i = 0; i < W->w.nb; ++i)

@@ -5,8 +5,10 @@ simulates only the bodies it owns.  What crosses NVLink is the north star's "all
     for proximity detection only; their states (13 floats: t3 q4 linvel3 angvel3) are all-gathered EVERY step and
     imported before the next one.  A rank with no halo takes part in no per-step collective at all.
   * every `refresh_every` (128) steps the owned states of ALL bodies are all-gathered, every rank re-derives its halo set
-    from them (bounding box of its own bodies, inflated by a margin that covers `refresh_every` steps at the fastest
-    body's current speed) and tells the others which of their bodies it now tracks.
+    from them (halo_rule: bounding box of its own bodies' reach spheres, inflated per axis by a margin that covers
+    `refresh_every` steps at the fastest body's current speed plus the largest acceleration gravity and user forces can
+    give) and tells the others which of their bodies it now tracks.  It also checks that no untracked body broke that
+    bound over the last window (check_bound), and raises HaloBoundError if one did.
   * a CONTACT between an owned and a halo body means two shards' islands merged: the device raises RB_ERR_SHARD
     (reported by the next synchronising call); nothing is silently simulated wrong.
   * `finish()` gathers everything once more, so all ranks end with the exact state of every body.
@@ -48,24 +50,104 @@ def state_tensor(pipe, device):
     return t.view(-1, 13)
 
 
-def body_radii(pipe):
-    """Bounding radius of each body about its origin (from the collider descriptors the pipeline uploaded)."""
-    r = np.zeros(pipe.nb, np.float32)
+def body_reach(pipe):
+    """(local centre of mass [nb, 3], reach [nb]) of every body: the radius about its centre of mass of a sphere that holds
+    every one of its colliders' broad-phase boxes (shape extent + the collider's offset from the centre of mass + its
+    contact skin + the prediction distance + the fat-box skin).  Centred on the centre of mass, the sphere is carried by
+    the body's linear velocity alone: spin turns the colliders inside it."""
+    from . import _abi as A
+    mp = pipe.debug_read("body_mprops", np.float32).reshape(-1, 16).astype(np.float64)
+    com = mp[:, 0:3]
+    prm = pipe.params
+    pad = (prm.normalized_prediction_distance + A.RB_FAT_SKIN_FACTOR) * prm.length_unit   # prediction distance + fat-box skin
+    r = np.zeros(pipe.nb, np.float64)
     for c in pipe._c:
         if c.parent < 0:
             continue
         he = np.array(c.half_extents[:], np.float64)
-        ext = float(he[0]) if c.shape == 0 else float(np.linalg.norm(he))
-        off = float(np.linalg.norm(np.array(c.pos_wrt_parent_t[:], np.float64)))
-        r[c.parent] = max(r[c.parent], off + ext)
-    return r
+        if c.shape == A.RB_SHAPE_BALL:
+            ext = he[0]
+        elif c.shape == A.RB_SHAPE_CUBOID:
+            ext = np.linalg.norm(he)
+        elif c.shape == A.RB_SHAPE_CAPSULE:      # (half height, radius, axis)
+            ext = he[0] + he[1]
+        elif c.shape == A.RB_SHAPE_CONVEX:       # (hull id, border radius)
+            ext = np.linalg.norm(pipe.hull_vertices[int(he[0]) - 1], axis=1).max() + he[1]
+        else:
+            raise ValueError(f"body_reach: unknown shape {c.shape}")
+        off = np.linalg.norm(np.array(c.pos_wrt_parent_t[:], np.float64) - com[c.parent])
+        r[c.parent] = max(r[c.parent], off + ext + c.contact_skin + pad)
+    return com.astype(np.float32), r.astype(np.float32)
+
+
+def rotate(q, v):
+    """v rotated by the unit quaternions q = (x, y, z, w), batched."""
+    b, w = q[:, 0:3], q[:, 3:4]
+    t = 2.0 * torch.cross(b, v, dim=1)
+    return v + w * t + torch.cross(b, t, dim=1)
+
+
+def body_centres(state, com):
+    """World centres of mass of the state rows [nb, 13] (translation, quaternion, linvel, angvel)."""
+    return state[:, 0:3] + rotate(state[:, 3:7], com)
+
+
+def owned_box(centre, reach, mine):
+    """Bounding box (lo [3], hi [3]) of the reach spheres of the bodies in `mine`, or None when there are none."""
+    if not bool(mine.any()):
+        return None
+    r = reach.unsqueeze(1)
+    return (centre - r)[mine].min(dim=0).values, (centre + r)[mine].max(dim=0).values
+
+
+def halo_margin(state, window, accel, min_margin=0.5):
+    """Per-axis margin [3] by which a rank's bounding box is widened: the owned and the foreign body can each cover
+    window * v_max + accel * window^2 / 2 before the next refresh, v_max the fastest body's speed now and accel the
+    per-axis bound on acceleration (gravity * max|gravity_scale| + max|F| / m)."""
+    lin = state[:, 7:10]
+    speed = lin.norm(dim=1).max() if lin.numel() else torch.zeros((), device=state.device)
+    return min_margin + 2.0 * window * speed + torch.as_tensor(accel, dtype=state.dtype, device=state.device) * window * window
+
+
+def halo_rule(state, com, reach, owner, rank, window, accel, min_margin=0.5):
+    """The foreign bodies rank `rank` must track for the next `window` seconds (uint8 mask [nb]): those whose reach
+    sphere meets the bounding box of its own bodies' reach spheres widened by halo_margin.  Before the next refresh no
+    untracked foreign body can come within the broad phase's reach of an owned one unless something the margin does not
+    bound (a contact impulse, a state edit, a kinematic target) accelerates it; IslandShard checks that at every refresh.
+    state [nb, 13], com [nb, 3], reach [nb], owner [nb] (int, -1 for fixed bodies) are tensors on one device."""
+    mine = owner == rank
+    foreign = (owner >= 0) & ~mine
+    centre = body_centres(state, com)
+    box = owned_box(centre, reach, mine)
+    if box is None:
+        return torch.zeros(owner.shape, dtype=torch.uint8, device=owner.device)
+    margin = halo_margin(state, window, accel, min_margin)
+    r = reach.unsqueeze(1)
+    near = ((centre + r >= box[0] - margin).all(dim=1) & (centre - r <= box[1] + margin).all(dim=1))
+    return (near & foreign).to(torch.uint8)
+
+
+def accel_bound(gravity, gravity_scale, user_force, inv_mass):
+    """Per-axis bound [3] on the acceleration of the given bodies: |gravity| times their largest |gravity_scale| plus
+    their largest |user force| * inverse mass (contact impulses are not bounded: IslandShard.check_bound)."""
+    if gravity is None:
+        raise ValueError("the halo margin needs the gravity: step the pipeline, build it through PhysicsWorld or pass gravity=")
+    g = np.abs(np.asarray(gravity, np.float64)) * float(np.abs(gravity_scale).max(initial=0.0))
+    return g + float((np.linalg.norm(user_force, axis=1) * inv_mass).max(initial=0.0))
+
+
+class HaloBoundError(RuntimeError):
+    """A foreign body reached a rank's bodies between two refreshes without being tracked there (see IslandShard)."""
 
 
 class IslandShard:
-    def __init__(self, pipe, dist, rank, world_size, device, refresh_every=128, min_margin=0.5, overlap=None):
+    def __init__(self, pipe, dist, rank, world_size, device, refresh_every=128, min_margin=0.5, overlap=None, gravity=None):
+        """gravity: the gravity the halo margin assumes; by default the one the pipeline was last stepped with (or given
+        by PhysicsWorld at construction), read at every refresh."""
         self.pipe, self.dist, self.rank, self.world_size, self.device = pipe, dist, rank, world_size, device
         self.refresh_every = int(refresh_every)
         self.min_margin = float(min_margin)
+        self.gravity = gravity
         self.dt = float(pipe.params.dt)
         self.tick = 0
         comp = pipe.label_components()
@@ -76,7 +158,12 @@ class IslandShard:
         owner_t = torch.from_numpy(self.owner.astype(np.int64)).to(device)
         self.mine = owner_t == rank
         self.foreign = (owner_t >= 0) & ~self.mine
-        self.radius = torch.from_numpy(body_radii(pipe)).to(device)
+        com, reach = body_reach(pipe)
+        self.com = torch.from_numpy(com).to(device)
+        self.reach = torch.from_numpy(reach).to(device)
+        self.moving = np.nonzero(self.owner >= 0)[0]
+        self.inv_mass = pipe.debug_read("body_mprops", np.float32).reshape(-1, 16)[self.moving, 3].astype(np.float64)
+        self.gravity_scale = np.array([pipe._b[b].gravity_scale for b in self.moving], np.float64)
         idx = [np.nonzero(self.owner == r)[0].astype(np.int64) for r in range(world_size)]
         self.counts = [len(i) for i in idx]
         self.maxc = max(max(self.counts), 1)
@@ -88,11 +175,16 @@ class IslandShard:
         self.other_idx = torch.cat([torch.from_numpy(idx[r]) for r in others] or [torch.zeros(0, dtype=torch.int64)]).to(device)
         self.other_rows = torch.cat([torch.arange(self.counts[r]) + r * self.maxc for r in others] or [torch.zeros(0, dtype=torch.int64)]).to(device)
         self.halo = torch.zeros(nb, dtype=torch.uint8, device=device)   # foreign bodies tracked here
+        self.masks = torch.zeros(world_size, nb, dtype=torch.uint8, device=device)   # every rank's halo
         self.owner_t = owner_t
         self.export_max = 0          # per-step halo exchange: rows per rank (0 = no per-step collective)
         self.halo_steps = 0          # steps that needed the per-step halo exchange (diagnostic)
         self.refreshes = 0
         self.refresh(classify=True, force=True)
+
+    def accel(self):
+        return accel_bound(self.pipe.gravity if self.gravity is None else self.gravity, self.gravity_scale,
+                           self.pipe.user_force[self.moving], self.inv_mass)
 
     # ---- full exchange (every refresh_every steps, at start-up and in finish) ----
     def _gather_all(self):
@@ -102,24 +194,38 @@ class IslandShard:
         if len(self.other_idx):
             self.state.index_copy_(0, self.other_idx, self.full_recv.index_select(0, self.other_rows))
 
+    def check_bound(self):
+        """After a full exchange: a foreign body that no rank's halo rule made it track over the last window and that now
+        lies within min_margin of a rank's owned bounding box on every axis broke the margin's bound (the margin keeps a
+        gap of at least min_margin on one axis otherwise).  Raises HaloBoundError naming the body; every rank holds the
+        same states and masks, so every rank raises.  A body that tunnelled through and ended apart is not seen."""
+        centre = body_centres(self.state, self.com)
+        r = self.reach.unsqueeze(1)
+        for rk in range(self.world_size):
+            mine = self.owner_t == rk
+            box = owned_box(centre, self.reach, mine)
+            if box is None:
+                continue
+            untracked = (self.owner_t >= 0) & ~mine & (self.masks[rk] == 0)
+            near = (centre + r >= box[0] - self.min_margin).all(dim=1) & (centre - r <= box[1] + self.min_margin).all(dim=1)
+            bad = torch.nonzero(near & untracked).flatten()
+            if bad.numel():
+                b = int(bad[0])
+                raise HaloBoundError(f"body {b} (rank {int(self.owner_t[b])}) reached the bodies of rank {rk} between two halo "
+                                     f"refreshes without being tracked there (after {self.tick} steps): its contacts may have been missed")
+
     def refresh(self, classify=True, force=False):
-        """All ranks get all states; each re-derives the bodies of other ranks it has to track (its halo) and, when any
-        rank's halo changed, learns which of its own bodies the others track (its exports).  One host synchronisation."""
+        """All ranks get all states; each checks that no untracked body broke the last window's bound, re-derives the
+        bodies of other ranks it has to track (its halo) and, when any rank's halo changed, learns which of its own bodies
+        the others track (its exports).  One host synchronisation."""
         self._gather_all()
+        if self.refreshes:
+            self.check_bound()
         if not classify:
             return
         self.refreshes += 1
-        pos, lin = self.state[:, 0:3], self.state[:, 7:10]
-        speed = lin.norm(dim=1).max() if lin.numel() else torch.zeros((), device=self.device)
-        margin = self.min_margin + 2.0 * self.refresh_every * self.dt * speed
-        r = self.radius.unsqueeze(1)
-        lo_all, hi_all = pos - r, pos + r
-        if bool(self.counts[self.rank]):
-            lo = lo_all[self.my_idx].min(dim=0).values - margin
-            hi = hi_all[self.my_idx].max(dim=0).values + margin
-            halo = ((hi_all >= lo).all(dim=1) & (lo_all <= hi).all(dim=1) & self.foreign).to(torch.uint8)
-        else:
-            halo = torch.zeros_like(self.halo)
+        halo = halo_rule(self.state, self.com, self.reach, self.owner_t, self.rank, self.refresh_every * self.dt,
+                         self.accel(), self.min_margin)
         changed = (halo != self.halo).any().to(torch.int32).reshape(1)
         self.dist.all_reduce(changed, op=self.dist.ReduceOp.MAX)
         if not force and int(changed.item()) == 0:     # (the host synchronisation of a refresh)
@@ -130,6 +236,7 @@ class IslandShard:
         # who tracks whom: all halo masks -> my export list and everybody's (for unpacking)
         masks = torch.zeros(self.world_size, self.halo.numel(), dtype=torch.uint8, device=self.device)
         self.dist.all_gather_into_tensor(masks.view(-1), self.halo)
+        self.masks = masks
         tracked = masks.any(dim=0)                      # bodies tracked by a rank other than their owner
         self.export_idx = []
         counts = []

@@ -29,6 +29,9 @@ class PhysicsPipeline:
             raise RapierError(self.L.rb_last_error().decode())
         self.nb = 0
         self._nhulls = 0
+        self.hull_vertices = []                # vertices [n, 3] of each registered hull (id = index + 1)
+        self.user_force = np.zeros((0, 3))     # the user force of every body as last set (sharding.py bounds accelerations with it)
+        self.gravity = None                    # the gravity of the last step (PhysicsWorld sets it at construction)
 
     def sync_hulls(self, colliders):
         """Registers the convex polyhedra the collider set has collected since the last call (rb_world_add_hull)."""
@@ -37,6 +40,7 @@ class PhysicsPipeline:
             verts, sizes, idx = hull_arrays(colliders.hulls[k])
             hid = self._check(self.L.rb_world_add_hull(self.h, len(verts), verts.ctypes.data, len(sizes), sizes.ctypes.data, idx.ctypes.data))
             assert hid == k + 1, (hid, k)
+            self.hull_vertices.append(verts.copy())
             self._nhulls = k + 1
 
     def close(self):
@@ -64,6 +68,7 @@ class PhysicsPipeline:
         self._j = as_array(joints.descs, A.RbJointDesc)
         self._check(self.L.rb_world_set_scene(self.h, len(bodies), self._b, len(colliders), self._c, len(joints), self._j))
         self.nb = len(bodies)
+        self.user_force = np.array([d.user_force[:] for d in bodies.descs], np.float64).reshape(-1, 3)
 
     def reserve(self, max_bodies, max_colliders):
         """Room for later insert() calls (applied by the next upload)."""
@@ -77,6 +82,7 @@ class PhysicsPipeline:
         fb, fc = C.c_int32(-1), C.c_int32(-1)
         self._check(self.L.rb_world_insert(self.h, len(body_descs), b, len(collider_descs), c, C.byref(fb), C.byref(fc)))
         self.nb += len(body_descs)
+        self.user_force = np.concatenate([self.user_force, np.array([d.user_force[:] for d in body_descs], np.float64).reshape(-1, 3)])
         return fb.value, fc.value
 
     def remove_bodies(self, indices):
@@ -116,11 +122,13 @@ class PhysicsPipeline:
         self._check(self.L.rb_world_set_params(self.h, C.byref(params)))
 
     def step(self, gravity, nsteps=1, sync=True):
+        self.gravity = tuple(gravity)
         g = (C.c_float * 3)(*gravity)
         self._check(self.L.rb_world_step(self.h, g, nsteps, 1 if sync else 0))
 
     def step_host(self, gravity, in_state13=None, out_state13=None):
         """PhysicsPipeline::step as a host-side owner of the sets calls it: host state in, host state out."""
+        self.gravity = tuple(gravity)
         g = (C.c_float * 3)(*gravity)
         self._check(self.L.rb_world_step_host(self.h, g,
                                               None if in_state13 is None else in_state13.ctypes.data,
@@ -156,6 +164,8 @@ class PhysicsPipeline:
         t = None if torque3 is None else np.ascontiguousarray(torque3, np.float32)
         self._check(self.L.rb_world_set_body_forces(self.h, len(idx), idx.ctypes.data, None if f is None else f.ctypes.data,
                                                     None if t is None else t.ctypes.data))
+        if f is not None:
+            self.user_force[idx] = f.reshape(-1, 3)
 
     def set_next_kinematic_positions(self, indices, pose7):
         """RigidBody::set_next_kinematic_position of position-based kinematic bodies ([n, 7]: translation, quaternion xyzw)."""
@@ -277,6 +287,7 @@ class PhysicsWorld:
         if scene is not None:
             self.gravity = scene.gravity
             self.bodies, self.colliders, self.impulse_joints = scene.bodies, scene.colliders, scene.joints
+        self.physics_pipeline.gravity = tuple(self.gravity)
 
     def reserve(self, max_bodies, max_colliders):
         """Capacity for bodies / colliders inserted after the first step (RigidBodySet / ColliderSet grow on demand in the
