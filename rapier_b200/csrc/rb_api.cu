@@ -30,6 +30,11 @@
 
 using namespace rb;
 
+// The kernels spell the public constants they share with the C ABI themselves (rb_world.cuh): they must agree.
+static_assert(STATUS_CAPACITY == RB_ERR_CAPACITY && STATUS_NONFINITE == RB_ERR_NONFINITE && STATUS_SHARD == RB_ERR_SHARD,
+              "device statuses are RbStatus values");
+static_assert(EV_COLLISION == RB_EVENT_COLLISION && EV_CONTACT_FORCE == RB_EVENT_CONTACT_FORCE, "c_events holds the RB_EVENT_* bits");
+
 // ------------------------------------------------------------------------------------------------
 // error handling + memory backend
 // ------------------------------------------------------------------------------------------------
@@ -922,7 +927,7 @@ static int sync_world(RbWorld* W, bool check = true) {
             W->host_hint[1] = 0;
             int zero = 0;
             CK(h2d(&W->w.st->error, &zero, sizeof(int)));
-            set_err(code == -6 ? "device raised status %d (a contact formed between bodies simulated by different ranks: the shards' islands merged, repartition)" : code == RB_ERR_NONFINITE ? "device raised status %d (non-finite body state: see rb_world_get_quarantine)"
+            set_err(code == RB_ERR_SHARD ? "device raised status %d (a contact formed between bodies simulated by different ranks: the shards' islands merged, repartition)" : code == RB_ERR_NONFINITE ? "device raised status %d (non-finite body state: see rb_world_get_quarantine)"
                                              : "device raised status %d (capacity overflow: the step kept the previous pair set / truncated the schedule)", code);
             return code;
         }
@@ -1050,7 +1055,7 @@ static int upload_colliders(RbWorld* W, int first, int count, int first_body = 0
     std::vector<float> thr(count);
     for (int k = 0; k < count; ++k) {
         const RbColliderDesc& c = W->colliders[first + k];
-        events[k] = (int)(c.active_events & 3u) | (c.sensor ? 4 : 0);
+        events[k] = (int)(c.active_events & (EV_COLLISION | EV_CONTACT_FORCE)) | (c.sensor ? EV_SENSOR : 0);
         if (c.sensor) w.has_sensors = 1;
         thr[k] = c.contact_force_event_threshold;
         if (c.active_events & RB_EVENT_CONTACT_FORCE) W->force_events = true;

@@ -172,7 +172,7 @@ RB_HD pose ccd_clamp_body(const World& w, int b, pose op, pose np, bool bullet =
     for (int c = w.b_col_head[b]; c >= 0; c = w.c_next[c]) {
         const int sh = w.c_shape[c];
         if (sh == SHAPE_REMOVED || sh >= SHAPE_CAPSULE) continue;   // (capsules and convex polyhedra are not swept: speculative contacts only)
-        if (w.has_sensors && (w.c_events[c] & 4)) continue;         // sensors neither sweep nor stop a sweep (ccd_solver.rs:92-93)
+        if (w.has_sensors && (w.c_events[c] & EV_SENSOR)) continue;   // sensors neither sweep nor stop a sweep (ccd_solver.rs:92-93)
         const vec3 he = xyz(w.c_he[c]);
         const pose rel = mkpose(mkq(w.c_rel_q[c]), xyz(w.c_rel_t[c]));
         const pose cs = pmul(op, rel), ce = pmul(np, rel);
@@ -188,7 +188,7 @@ RB_HD pose ccd_clamp_body(const World& w, int b, pose op, pose np, bool bullet =
             const int pj = w.c_parent[cj];
             if (pj >= 0 && w.b_type[pj] != BODY_FIXED) return;   // tier_allows (sweeps.rs:36-42): non-bullets only hit fixed targets
             if (w.c_shape[cj] >= SHAPE_CAPSULE) return;
-            if (w.has_sensors && (w.c_events[cj] & 4)) return;
+            if (w.has_sensors && (w.c_events[cj] & EV_SENSOR)) return;
             if (!ccd_groups_allow(w, c, cj, g1)) return;
             const float f = ccd_toi(w.c_shape[cj], xyz(w.c_he[cj]), collider_pose(w, cj), sh, he, sw, slop);
             if (f > 0.0f && f < frac) frac = f;
@@ -203,7 +203,7 @@ RB_HD pose ccd_clamp_body(const World& w, int b, pose op, pose np, bool bullet =
                 const int pj = w.c_parent[cj], shj = w.c_shape[cj];
                 if (pj == b || pj < 0 || shj == SHAPE_REMOVED || shj >= SHAPE_CAPSULE) continue;
                 if (!type_is_solver(w.b_type[pj])) continue;
-                if (w.has_sensors && (w.c_events[cj] & 4)) continue;
+                if (w.has_sensors && (w.c_events[cj] & EV_SENSOR)) continue;
                 if (w.b_type[pj] == BODY_DYNAMIC && (w.b_flags[pj] & FLAG_CCD)) continue;
                 if (!fat_overlap(amin, amax, w.c_fat_min[cj], w.c_fat_max[cj])) continue;
                 if (!ccd_groups_allow(w, c, cj, g1)) continue;

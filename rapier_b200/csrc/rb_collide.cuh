@@ -292,13 +292,19 @@ RB_HD void clear_color_bits(const World& w, int color, int cb0, int cb1) {
         if (cb1 >= 0) atomic_and(&w.color_mask[cb1 * 4 + (color >> 5)], bit);
     }
 }
+// A touching pair that stops being a constraint gives its colour back: the bit on its colour bodies, then the colour itself.
+RB_HD void drop_pair_color(const World& w, int buf, int i, float4 bod, int& color) {
+    clear_color_bits(w, color, as_int(bod.x), as_int(bod.y));
+    color = COLOR_UNCOLORED;
+    prow(w, buf, PR_BODIES, i) = make_float4(as_float_i(-1), as_float_i(-1), bod.z, bod.w);
+}
 
 // EventHandler::handle_collision_event (contacts.rs:312-324): buffered for the host when either collider asks for it.
 RB_HD void emit_collision_event(const World& w, int c1, int c2, bool started) {
-    if (!((w.c_events[c1] | w.c_events[c2]) & 1)) return;
+    if (!((w.c_events[c1] | w.c_events[c2]) & EV_COLLISION)) return;
     const int slot = atomic_add(&w.st->nev_coll, 1);
     if (slot < w.ev_cap) w.ev_coll[slot] = make_int4(c1, c2, started ? 1 : 0, w.step_index);
-    else RB_RAISE(w, -4);
+    else RB_RAISE(w, STATUS_CAPACITY);
 }
 
 RB_HD bool collider_is_static(const World& w, int c) {   // never moves: no parent, or a parent that is neither dynamic nor kinematic
@@ -348,7 +354,7 @@ RB_PHASE void section_fixed_pairs(const Ctx& ctx, const World& w, const unsigned
         for (int k = 0; k < nwide; ++k) test(w.wide_list[k]);
     }
     ctx.grid_sync();
-    if (ctx.gtid == 0 && st->nff > w.pair_cap) RB_RAISE(w, -4);   // (the list keeps what fits; the status reports the rest)
+    if (ctx.gtid == 0 && st->nff > w.pair_cap) RB_RAISE(w, STATUS_CAPACITY);   // (the list keeps what fits; the status reports the rest)
 }
 
 // P1 (lists): split the colliders into the movers (sorted every time an AABB changes) and the static ones (sorted
@@ -513,7 +519,7 @@ RB_PHASE void section_broad_phase(const Ctx& ctx, const World& w) {
     const int ncand = st->ncand;
     if (ncand > w.pair_cap) {  // capacity overflow: keep the old pair set and raise the status; the pair set stays dirty,
                                // so every step raises it again until the world fits (no silently stale physics)
-        if (ctx.gtid == 0) RB_RAISE(w, -4);
+        if (ctx.gtid == 0) RB_RAISE(w, STATUS_CAPACITY);
         ctx.grid_sync();
         return;
     }
@@ -566,7 +572,7 @@ RB_PHASE void section_broad_phase(const Ctx& ctx, const World& w) {
     for (int j = ctx.gtid; j < nold; j += ctx.gsize) {
         if (bsearch_u64(ck, ncand, okey[j]) < 0) {
             float4 info = prow(w, cur, PR_INFO, j), bod = prow(w, cur, PR_BODIES, j);
-            if (as_int(info.z) > 0 || (as_int(info.x) & 16)) emit_collision_event(w, (int)(okey[j] >> 32), (int)(okey[j] & 0xffffffffu), false);   // a touching (or intersecting sensor) pair that leaves the broad phase stops
+            if (as_int(info.z) > 0 || (as_int(info.x) & PF_SENSOR_HIT)) emit_collision_event(w, (int)(okey[j] >> 32), (int)(okey[j] & 0xffffffffu), false);   // a touching (or intersecting sensor) pair that leaves the broad phase stops
             clear_color_bits(w, as_int(info.w), as_int(bod.x), as_int(bod.y));
         }
     }
@@ -658,8 +664,8 @@ RB_PHASE void phase_convex_manifolds(const Ctx& ctx, const World& w) {
         if (!pair_is_poly_poly(w.c_shape[c1], w.c_shape[c2])) continue;
         const float4 bod0 = prow(w, buf, PR_BODIES, i);
         const int flags = as_int(prow(w, buf, PR_INFO, i).x);
-        if (!body_is_sim(w, as_int(bod0.z)) && !body_is_sim(w, as_int(bod0.w)) && !(w.has_filters && !(flags & 64))) continue;
-        if (recycle > 0.0f && (flags & 1)) {
+        if (!body_is_sim(w, as_int(bod0.z)) && !body_is_sim(w, as_int(bod0.w)) && !(w.has_filters && !(flags & PF_UPDATED))) continue;
+        if (recycle > 0.0f && (flags & PF_RECYCLE)) {
             const pose cp1 = collider_pose(w, c1), cp2 = collider_pose(w, c2);
             const pose p12 = pinv_mul(cp1, cp2);
             const float4 rt = prow(w, buf, PR_RT, i);
@@ -712,7 +718,7 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
             // static colliders, or a pair that a filter change brought back under a sleeping body)
             float4 bod0 = prow(w, buf, PR_BODIES, i);
             if (!body_is_sim(w, as_int(bod0.z)) && !body_is_sim(w, as_int(bod0.w)) &&
-                !(w.has_filters && !(as_int(prow(w, buf, PR_INFO, i).x) & 64)))
+                !(w.has_filters && !(as_int(prow(w, buf, PR_INFO, i).x) & PF_UPDATED)))
                 continue;
         }
         pose cp1 = collider_pose(w, c1), cp2 = collider_pose(w, c2);
@@ -725,7 +731,7 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
             forceless = pair_forceless(w, c1, c2, as_int(bodf.z), as_int(bodf.w));
         }
         // contact recycling (pair_update.rs:111-171); a pair whose solver outcome changed is recomputed (:116-121)
-        if (recycle > 0.0f && (flags & 1) && forceless == ((flags & 32) != 0)) {
+        if (recycle > 0.0f && (flags & PF_RECYCLE) && forceless == ((flags & PF_FORCELESS) != 0)) {
             float4 rt = prow(w, buf, PR_RT, i);
             pose base = mkpose(mkq(prow(w, buf, PR_RQ, i)), xyz(rt));
             float drift = pose_drift(base, p12, rt.w);
@@ -743,13 +749,13 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
         if (SHAPES && pair_is_poly_poly(sh1, sh2)) poly_raw_load(w.convex_raw + (size_t)i * POLY_RAW_STRIDE, raw);   // (phase_convex_manifolds)
         else contact_manifold<SHAPES>(w.hulls, sh1, he1, sh2, he2, p12, prediction + (skin1 + skin2), raw);
 
-        if (w.has_sensors && ((w.c_events[c1] | w.c_events[c2]) & 4)) {   // (a kernel parameter guards the loads)
+        if (w.has_sensors && ((w.c_events[c1] | w.c_events[c2]) & EV_SENSOR)) {   // (a kernel parameter guards the loads)
             // a pair with a sensor (narrow_phase/intersections.rs:17-221): no contacts, no colour, no island edge -- only whether
             // the shapes intersect (the deepest manifold point is not positive), with a CollisionEvent when that changes
             bool inter = false;
             for (int k = 0; k < raw.n; ++k) inter = inter || raw.pt[k].dist <= 0.0f;
-            if (inter != ((flags & 16) != 0)) emit_collision_event(w, c1, c2, inter);
-            prow(w, buf, PR_INFO, i) = make_float4(as_float_i((inter ? 16 : 0) | (w.has_filters ? 64 : 0)), as_float_i(0), as_float_i(0), as_float_i(color));
+            if (inter != ((flags & PF_SENSOR_HIT) != 0)) emit_collision_event(w, c1, c2, inter);
+            prow(w, buf, PR_INFO, i) = make_float4(as_float_i((inter ? PF_SENSOR_HIT : 0) | (w.has_filters ? PF_UPDATED : 0)), as_float_i(0), as_float_i(0), as_float_i(color));
             continue;
         }
 
@@ -843,9 +849,9 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
         }
         float max_drift = 0.0f;
         if (recycle > 0.0f) {  // pair_update.rs:582-613
-            float max_extent = (flags & 1) ? prow(w, buf, PR_RT, i).w : max2(origin_radius(w, sh1, he1), origin_radius(w, sh2, he2));
+            float max_extent = (flags & PF_RECYCLE) ? prow(w, buf, PR_RT, i).w : max2(origin_radius(w, sh1, he1), origin_radius(w, sh2, he2));
             max_drift = nsc > 0 ? recycle : min2(recycle, prediction);
-            flags |= 1;
+            flags |= PF_RECYCLE;
             prow(w, buf, PR_RT, i) = f4(p12.t, max_extent);
             prow(w, buf, PR_RQ, i) = f4(p12.q);
             prow(w, buf, PR_ROT1, i) = f4(cp1.q);
@@ -858,40 +864,36 @@ RB_PHASE void phase_narrow_phase(const Ctx& ctx, const World& w) {
         bool had = nsc_old > 0, has = nsc > 0;
         if (has && dyn1 != dyn2) {   // sharding: a contact with a body simulated by ANOTHER rank means two shards' islands merged
             const int bo = dyn1 ? b2 : b1;
-            if (bo >= 0 && w.b_type[bo] == BODY_DYNAMIC && w.b_owned[bo] != 1) RB_RAISE(w, -6);
+            if (bo >= 0 && w.b_type[bo] == BODY_DYNAMIC && w.b_owned[bo] != 1) RB_RAISE(w, STATUS_SHARD);
         }
         if (had != has) {
             st->sched_dirty = 1;
             emit_collision_event(w, c1, c2, has);
-            if (!has) flags &= ~8;   // the force-event status resets when the colliders separate (geometry/mod.rs:208-217)
+            if (!has) flags &= ~PF_FORCE_EVENT;   // the force-event status resets when the colliders separate (geometry/mod.rs:208-217)
             if (has) {
                 if (!forceless) {
-                    flags |= 2;  // pending colour (deferred greedy pass)
+                    flags |= PF_PENDING_COLOR;
                     st->ntodo = 1;
                 }
                 // a contact that begins wakes the sleeping side's whole island (narrow_phase/mod.rs:53-67)
                 if (dyn1 && w.b_sleeping[b1]) { w.wake_req[w.isl_label[b1]] = 1; st->wake_any = 1; }
                 if (dyn2 && w.b_sleeping[b2]) { w.wake_req[w.isl_label[b2]] = 1; st->wake_any = 1; }
             } else {
-                clear_color_bits(w, color, as_int(bod.x), as_int(bod.y));
-                color = COLOR_UNCOLORED;
-                prow(w, buf, PR_BODIES, i) = make_float4(as_float_i(-1), as_float_i(-1), bod.z, bod.w);
+                drop_pair_color(w, buf, i, bod, color);
             }
         }
         if (w.has_filters) {
-            if (had && has && forceless != ((flags & 32) != 0)) {   // a touching pair gains or loses its forces: recolour, reschedule
+            if (had && has && forceless != ((flags & PF_FORCELESS) != 0)) {   // a touching pair gains or loses its forces: recolour, reschedule
                 st->sched_dirty = 1;
                 if (forceless) {
-                    clear_color_bits(w, color, as_int(bod.x), as_int(bod.y));
-                    color = COLOR_UNCOLORED;
-                    flags &= ~8;
-                    prow(w, buf, PR_BODIES, i) = make_float4(as_float_i(-1), as_float_i(-1), bod.z, bod.w);
+                    flags &= ~PF_FORCE_EVENT;
+                    drop_pair_color(w, buf, i, bod, color);
                 } else {
-                    flags |= 2;
+                    flags |= PF_PENDING_COLOR;
                     st->ntodo = 1;
                 }
             }
-            flags = (forceless ? (flags | 32) : (flags & ~32)) | 64;
+            flags = (forceless ? (flags | PF_FORCELESS) : (flags & ~PF_FORCELESS)) | PF_UPDATED;
         }
         prow(w, buf, PR_INFO, i) = make_float4(as_float_i(flags), as_float_i(nsel), as_float_i(nsc), as_float_i(color));
     }
@@ -942,7 +944,7 @@ RB_PHASE void section_coloring(const Ctx& ctx, const World& w) {
     // this list, not the whole pair table (a settling pile runs dozens of rounds over a few thousand pending pairs)
     int* list = w.cons_pair_tmp;
     for (int i = ctx.gtid; i < np; i += ctx.gsize)
-        if (as_int(prow(w, buf, PR_INFO, i).x) & 2) list[atomic_add(&st->ncand, 1)] = i;   // (ncand: 0 outside the broad phase)
+        if (as_int(prow(w, buf, PR_INFO, i).x) & PF_PENDING_COLOR) list[atomic_add(&st->ncand, 1)] = i;   // (ncand: 0 outside the broad phase)
     ctx.grid_sync();
     const int nlist = st->ncand < w.cons_cap ? st->ncand : w.cons_cap;
     ctx.grid_sync();
@@ -953,7 +955,7 @@ RB_PHASE void section_coloring(const Ctx& ctx, const World& w) {
         for (int k = ctx.gtid; k < nlist; k += ctx.gsize) {
             const int i = list[k];
             int flags = as_int(prow(w, buf, PR_INFO, i).x);
-            if (!(flags & 2)) continue;
+            if (!(flags & PF_PENDING_COLOR)) continue;
             float4 bod = prow(w, buf, PR_BODIES, i);
             int b1 = as_int(bod.z), b2 = as_int(bod.w);
             const unsigned long long key = color_order_key(b1, b2);
@@ -968,7 +970,7 @@ RB_PHASE void section_coloring(const Ctx& ctx, const World& w) {
         for (int k = ctx.gtid; k < nlist; k += ctx.gsize) {
             const int i = list[k];
             int flags = as_int(prow(w, buf, PR_INFO, i).x);
-            if (!(flags & 2)) continue;
+            if (!(flags & PF_PENDING_COLOR)) continue;
             float4 bod = prow(w, buf, PR_BODIES, i);
             int b1 = as_int(bod.z), b2 = as_int(bod.w);
             const unsigned long long key = color_order_key(b1, b2);
@@ -981,7 +983,7 @@ RB_PHASE void section_coloring(const Ctx& ctx, const World& w) {
             const int i = list[k];
             float4 info = prow(w, buf, PR_INFO, i);
             int flags = as_int(info.x);
-            if (!(flags & 2)) continue;
+            if (!(flags & PF_PENDING_COLOR)) continue;
             float4 bod = prow(w, buf, PR_BODIES, i);
             int b1 = as_int(bod.z), b2 = as_int(bod.w);
             bool d1 = body_is_dyn(w, b1), d2 = body_is_dyn(w, b2);
@@ -1002,7 +1004,7 @@ RB_PHASE void section_coloring(const Ctx& ctx, const World& w) {
                 if (cb1 >= 0) w.color_mask[cb1 * 4 + (color >> 5)] |= 1u << (color & 31);
             }
             prow(w, buf, PR_BODIES, i) = make_float4(as_float_i(cb0), as_float_i(cb1), bod.z, bod.w);
-            info.x = as_float_i((flags & ~2) | 4);  // bit2: coloured this round (scratch reset below)
+            info.x = as_float_i((flags & ~PF_PENDING_COLOR) | PF_COLORED);   // (scratch reset below)
             info.w = as_float_i(color);
             prow(w, buf, PR_INFO, i) = info;
         }
@@ -1012,12 +1014,12 @@ RB_PHASE void section_coloring(const Ctx& ctx, const World& w) {
             const int i = list[k];
             float4 info = prow(w, buf, PR_INFO, i);
             int flags = as_int(info.x);
-            if (!(flags & 6)) continue;
+            if (!(flags & (PF_PENDING_COLOR | PF_COLORED))) continue;
             float4 bod = prow(w, buf, PR_BODIES, i);
             int b1 = as_int(bod.z), b2 = as_int(bod.w);
             if (body_is_dyn(w, b1)) { w.body_min[b1] = 0x7fffffff; w.body_minkey[b1] = ~0ull; }
             if (body_is_dyn(w, b2)) { w.body_min[b2] = 0x7fffffff; w.body_minkey[b2] = ~0ull; }
-            if (flags & 4) { info.x = as_float_i(flags & ~4); prow(w, buf, PR_INFO, i) = info; }
+            if (flags & PF_COLORED) { info.x = as_float_i(flags & ~PF_COLORED); prow(w, buf, PR_INFO, i) = info; }
         }
         if (ctx.gtid == 0) st->ncand = 0;
         ctx.grid_sync();
@@ -1197,6 +1199,75 @@ RB_PHASE void section_sleep(const Ctx& ctx, const World& w) {
     ctx.grid_sync();
 }
 
+// ---- the schedule's per-constraint rules ----
+// A touching pair is a constraint unless its contacts have no forces (worlds with collider filters).
+RB_HD bool pair_has_forces(const World& w, float4 info) {
+    return as_int(info.z) > 0 && !(w.has_filters && (as_int(info.x) & PF_FORCELESS));
+}
+// The awake body simulated here through which a pair or joint joins an island (both of its ends share it), or -1.
+RB_HD int island_body(const World& w, int b1, int b2) { return body_is_sim(w, b1) ? b1 : (body_is_sim(w, b2) ? b2 : -1); }
+// An island above either cap of a work item goes to the grid-wide item 0 ...
+RB_HD bool island_is_large(int nbod, int ncon) { return nbod > ITEM_BODY_CAP || ncon > ITEM_CONS_CAP; }
+// ... and adds nothing to the cost of the others, max(bodies, constraints) per island.
+RB_HD int island_cost(int nbod, int ncon) { return island_is_large(nbod, ncon) ? 0 : (nbod > ncon ? nbod : ncon); }
+// Launch-order bucket of work item `it` (1..): the most expensive items, max(bodies, contacts + joints), come first; -1 = empty.
+RB_HD int item_order_bucket(const World& w, int it) {
+    const int nbod = w.item_body_start[it + 1] - w.item_body_start[it];
+    const int work = (w.item_cons_start[it + 1] - w.item_cons_start[it]) + (w.item_joint_start[it + 1] - w.item_joint_start[it]);
+    if (nbod == 0 && work == 0) return -1;
+    const int cost = nbod > work ? nbod : work;
+    return ORDER_BUCKETS - 1 - (cost < ORDER_BUCKETS ? cost : ORDER_BUCKETS - 1);
+}
+// A colour above COLOR_OVERFLOW (COLOR_UNCOLORED) is solved in the overflow stage.
+RB_HD int clamp_color(int color) { return color > COLOR_OVERFLOW ? COLOR_OVERFLOW : color; }
+RB_HD void insertion_sort(int* a, int n) {
+    for (int x = 1; x < n; ++x) {
+        int v = a[x], y = x;
+        while (y > 0 && a[y - 1] > v) { a[y] = a[y - 1]; --y; }
+        a[y] = v;
+    }
+}
+// The contact or the joint tables of the per-item schedule.
+struct SchedSide {
+    bool joints;
+    const int* starts;   // item segments (item_cons_start / item_joint_start)
+    const int* src;      // ids grouped by item (cons_pair_tmp / joint_tmp)
+    int* dst;            // ids in stage order (cons_pair / joint_sched)
+    int* offs;           // [item_cap][NUM_COLORS + 1] stage offsets relative to the item's start (item_color_off / item_jcolor_off)
+    const int* cpos;     // stage position of a colour (color_pos / jcolor_pos)
+    RB_HD int stage(const World& w, int buf, int id) const {
+        return cpos[clamp_color(joints ? w.j_info[id].w : as_int(prow(w, buf, PR_INFO, id).w))];
+    }
+};
+RB_HD SchedSide sched_side(const World& w, bool joints) {
+    if (joints) return {true, w.item_joint_start, w.joint_tmp, w.joint_sched, w.item_jcolor_off, w.jcolor_pos};
+    return {false, w.item_cons_start, w.cons_pair_tmp, w.cons_pair, w.item_color_off, w.color_pos};
+}
+// Header of the constraint `id` in schedule slot q: its two awake bodies (global ids, or their index inside the item with
+// `local`; NO_BODY for any other body) and its island's substep key.  A contact then leaves its dominating side
+// world-attached (contact_with_twist_friction.rs:71-84).
+RB_HD void write_sched_header(const World& w, int buf, bool joints, bool local, int q, int id) {
+    int b1, b2;
+    if (!joints) {
+        const float4 bod = prow(w, buf, PR_BODIES, id);
+        b1 = as_int(bod.z); b2 = as_int(bod.w);
+    } else {
+        const int4 ji = w.j_info[id];
+        b1 = ji.x; b2 = ji.y;
+    }
+    int id1 = body_is_sim(w, b1) ? (local ? w.body_local[b1] : b1) : NO_BODY;
+    int id2 = body_is_sim(w, b2) ? (local ? w.body_local[b2] : b2) : NO_BODY;
+    if (w.any_extra) (joints ? w.j_key : w.cons_key)[q] = w.b_key[id1 != NO_BODY ? b1 : b2];   // (both ends share the island)
+    if (joints) {
+        w.j_sched_ids[q] = make_int4(id, id1, id2, 0);
+        return;
+    }
+    const int rel_dom = relative_dominance(w, b1, b2);
+    if (rel_dom > 0) id1 = NO_BODY;
+    if (rel_dom < 0) id2 = NO_BODY;
+    w.cons_hdr[q] = make_int4(id, id1, id2, 0);
+}
+
 // P3b: work items, colour stage order (init.rs:163-254) and the per-item constraint schedule of the AWAKE islands.
 template <class Ctx>
 RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
@@ -1222,19 +1293,17 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
             if (extra != 0u && body_is_sim(w, b)) atomic_max_u(&w.isl_key[w.isl_label[b]], extra);
         }
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
-        float4 info = prow(w, buf, PR_INFO, i);
-        if (as_int(info.z) <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;   // (forceless pairs are no constraint)
-        float4 bod = prow(w, buf, PR_BODIES, i);
-        int b1 = as_int(bod.z), b2 = as_int(bod.w);
-        int b = body_is_sim(w, b1) ? b1 : (body_is_sim(w, b2) ? b2 : -1);
+        const float4 info = prow(w, buf, PR_INFO, i);
+        if (!pair_has_forces(w, info)) continue;
+        const float4 bod = prow(w, buf, PR_BODIES, i);
+        const int b = island_body(w, as_int(bod.z), as_int(bod.w));
         if (b < 0) continue;
         atomic_add(&w.isl_ncons[w.isl_label[b]], 1);
-        int color = as_int(info.w);
-        atomic_add(&w.color_count[color > COLOR_OVERFLOW ? COLOR_OVERFLOW : color], 1);
+        atomic_add(&w.color_count[clamp_color(as_int(info.w))], 1);
     }
     for (int j = ctx.gtid; j < nj; j += ctx.gsize) {
-        int4 ji = w.j_info[j];
-        int b = body_is_sim(w, ji.x) ? ji.x : (body_is_sim(w, ji.y) ? ji.y : -1);
+        const int4 ji = w.j_info[j];
+        const int b = island_body(w, ji.x, ji.y);
         if (b >= 0) atomic_add(&w.isl_ncons[w.isl_label[b]], 1);
     }
     ctx.grid_sync();
@@ -1270,11 +1339,7 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
     int* cost = w.isl_item;  // reuse as input, overwritten by the item id below
     for (int b = ctx.gtid; b < nb; b += ctx.gsize) {
         int c = 0;
-        if (body_is_sim(w, b) && w.isl_label[b] == b) {
-            int nbod = w.isl_nb[b], ncon = w.isl_ncons[b];
-            bool large = nbod > ITEM_BODY_CAP || ncon > ITEM_CONS_CAP;
-            c = large ? 0 : (nbod > ncon ? nbod : ncon);
-        }
+        if (body_is_sim(w, b) && w.isl_label[b] == b) c = island_cost(w.isl_nb[b], w.isl_ncons[b]);
         cost[b] = c;
     }
     ctx.grid_sync();
@@ -1282,15 +1347,13 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
     int total_cost = w.scan_tmp[ctx.gsize];
     int nitems = 1 + (total_cost + ITEM_TARGET - 1) / ITEM_TARGET;
     if (nitems > w.item_cap) {
-        if (ctx.gtid == 0) RB_RAISE(w, -4);
+        if (ctx.gtid == 0) RB_RAISE(w, STATUS_CAPACITY);
         nitems = w.item_cap;
     }
     for (int b = ctx.gtid; b < nb; b += ctx.gsize) {
         int it = -1;
         if (body_is_sim(w, b) && w.isl_label[b] == b) {
-            int nbod = w.isl_nb[b], ncon = w.isl_ncons[b];
-            bool large = nbod > ITEM_BODY_CAP || ncon > ITEM_CONS_CAP;
-            it = large ? 0 : 1 + w.body_item[b] / ITEM_TARGET;
+            it = island_is_large(w.isl_nb[b], w.isl_ncons[b]) ? 0 : 1 + w.body_item[b] / ITEM_TARGET;
             if (it >= nitems) it = nitems - 1;
         }
         w.isl_item[b] = it;
@@ -1305,16 +1368,14 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         if (w.any_extra) w.b_key[b] = (unsigned char)(it >= 0 ? w.isl_key[w.isl_label[b]] : 0u);
     }
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
-        const float4 info = prow(w, buf, PR_INFO, i);
-        if (as_int(info.z) <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;
-        float4 bod = prow(w, buf, PR_BODIES, i);
-        int b1 = as_int(bod.z), b2 = as_int(bod.w);
-        int b = body_is_sim(w, b1) ? b1 : (body_is_sim(w, b2) ? b2 : -1);
+        if (!pair_has_forces(w, prow(w, buf, PR_INFO, i))) continue;
+        const float4 bod = prow(w, buf, PR_BODIES, i);
+        const int b = island_body(w, as_int(bod.z), as_int(bod.w));
         if (b >= 0) atomic_add(&w.item_cons_start[w.isl_item[w.isl_label[b]]], 1);
     }
     for (int j = ctx.gtid; j < nj; j += ctx.gsize) {
-        int4 ji = w.j_info[j];
-        int b = body_is_sim(w, ji.x) ? ji.x : (body_is_sim(w, ji.y) ? ji.y : -1);
+        const int4 ji = w.j_info[j];
+        const int b = island_body(w, ji.x, ji.y);
         if (b >= 0) atomic_add(&w.item_joint_start[w.isl_item[w.isl_label[b]]], 1);
     }
     ctx.grid_sync();
@@ -1325,7 +1386,7 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
     grid_exclusive_scan(ctx, w.item_joint_start, w.item_joint_start, nitems + 1, w.scan_tmp);
     int ncons = w.item_cons_start[nitems];
     if (ncons > w.cons_cap) {
-        if (ctx.gtid == 0) RB_RAISE(w, -4);
+        if (ctx.gtid == 0) RB_RAISE(w, STATUS_CAPACITY);
     }
     RB_CSTAMP(12);
     // S9 scatter bodies / manifolds / joints into their item segments
@@ -1340,11 +1401,9 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         w.body_local[b] = l;
     }
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
-        const float4 info = prow(w, buf, PR_INFO, i);
-        if (as_int(info.z) <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;
-        float4 bod = prow(w, buf, PR_BODIES, i);
-        int b1 = as_int(bod.z), b2 = as_int(bod.w);
-        int b = body_is_sim(w, b1) ? b1 : (body_is_sim(w, b2) ? b2 : -1);
+        if (!pair_has_forces(w, prow(w, buf, PR_INFO, i))) continue;
+        const float4 bod = prow(w, buf, PR_BODIES, i);
+        const int b = island_body(w, as_int(bod.z), as_int(bod.w));
         if (b < 0) continue;
         int it = w.body_item[b];
         int l = atomic_add(&cur_c[it], 1);
@@ -1352,8 +1411,8 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         if (pos < w.cons_cap) w.cons_pair_tmp[pos] = i;
     }
     for (int j = ctx.gtid; j < nj; j += ctx.gsize) {
-        int4 ji = w.j_info[j];
-        int b = body_is_sim(w, ji.x) ? ji.x : (body_is_sim(w, ji.y) ? ji.y : -1);
+        const int4 ji = w.j_info[j];
+        const int b = island_body(w, ji.x, ji.y);
         if (b < 0) continue;
         int it = w.body_item[b];
         int l = atomic_add(&cur_j[it], 1);
@@ -1370,18 +1429,14 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         RB_SHARED int offs0[NUM_COLORS + 1];
         RB_SHARED int base0[NUM_COLORS + 1];
         RB_SHARED int curs0[NUM_COLORS + 1];
-        const int* starts = pass == 0 ? w.item_cons_start : w.item_joint_start;
-        const int s0 = starts[0];
-        int s1 = starts[1];
+        const SchedSide t = sched_side(w, pass == 1);
+        const int s0 = t.starts[0];
+        int s1 = t.starts[1];
         if (pass == 0 && s1 > w.cons_cap) s1 = s0 > w.cons_cap ? s0 : w.cons_cap;
-        const int* src = pass == 0 ? w.cons_pair_tmp : w.joint_tmp;
-        int* dst = pass == 0 ? w.cons_pair : w.joint_sched;
-        int* offs = pass == 0 ? w.item_color_off : w.item_jcolor_off;   // (item 0's row)
-        const int* cpos = pass == 0 ? w.color_pos : w.jcolor_pos;
         int* ghist = w.order_hist;                       // [NUM_COLORS + 1] totals   (order_hist is free until S11)
         int* gcurs = w.order_hist + (NUM_COLORS + 1);    // [NUM_COLORS + 1] running bases of the CTAs
         if (s1 <= s0) {   // (uniform) nothing in item 0: an empty colour table
-            for (int c = ctx.gtid; c <= NUM_COLORS; c += ctx.gsize) offs[c] = 0;
+            for (int c = ctx.gtid; c <= NUM_COLORS; c += ctx.gsize) t.offs[c] = 0;
             continue;
         }
         for (int c = ctx.gtid; c < 2 * (NUM_COLORS + 1); c += ctx.gsize) ghist[c] = 0;
@@ -1390,12 +1445,7 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         const int n0 = s1 - s0;
         const int chunk = (n0 + ctx.nblocks - 1) / ctx.nblocks;
         const int q0 = s0 + ctx.bid * chunk, q1 = q0 + chunk < s1 ? q0 + chunk : s1;
-        for (int q = q0 + ctx.btid; q < q1; q += ctx.bsize) {
-            const int id = src[q];
-            int color = pass == 0 ? as_int(prow(w, buf, PR_INFO, id).w) : w.j_info[id].w;
-            if (color > COLOR_OVERFLOW) color = COLOR_OVERFLOW;
-            atomic_add(&hist0[cpos[color]], 1);
-        }
+        for (int q = q0 + ctx.btid; q < q1; q += ctx.bsize) atomic_add(&hist0[t.stage(w, buf, t.src[q])], 1);
         ctx.block_sync();
         for (int c = ctx.btid; c < NUM_COLORS; c += ctx.bsize)
             if (hist0[c] > 0) atomic_add(&ghist[c], hist0[c]);
@@ -1411,47 +1461,19 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         }
         ctx.block_sync();
         if (ctx.bid == 0)
-            for (int c = ctx.btid; c <= NUM_COLORS; c += ctx.bsize) offs[c] = offs0[c];
+            for (int c = ctx.btid; c <= NUM_COLORS; c += ctx.bsize) t.offs[c] = offs0[c];
         for (int q = q0 + ctx.btid; q < q1; q += ctx.bsize) {
-            const int id = src[q];
-            int color = pass == 0 ? as_int(prow(w, buf, PR_INFO, id).w) : w.j_info[id].w;
-            if (color > COLOR_OVERFLOW) color = COLOR_OVERFLOW;
-            const int p = cpos[color];
-            dst[s0 + offs0[p] + base0[p] + atomic_add(&curs0[p], 1)] = id;
+            const int id = t.src[q];
+            const int p = t.stage(w, buf, id);
+            t.dst[s0 + offs0[p] + base0[p] + atomic_add(&curs0[p], 1)] = id;
         }
         ctx.grid_sync();
-        if (ctx.gtid == 0 && cpos[COLOR_OVERFLOW] >= 0) {   // the overflow colour is solved sequentially: order it by index
-            const int p = cpos[COLOR_OVERFLOW];
-            const int a = s0 + offs0[p], e = s0 + offs0[p + 1];
-            for (int x = a + 1; x < e; ++x) {
-                int v = dst[x], y = x;
-                while (y > a && dst[y - 1] > v) { dst[y] = dst[y - 1]; --y; }
-                dst[y] = v;
-            }
+        if (ctx.gtid == 0 && t.cpos[COLOR_OVERFLOW] >= 0) {   // the overflow colour is solved sequentially: order it by index
+            const int p = t.cpos[COLOR_OVERFLOW];
+            insertion_sort(t.dst + s0 + offs0[p], offs0[p + 1] - offs0[p]);
         }
         ctx.grid_sync();
-        for (int q = s0 + ctx.gtid; q < s1; q += ctx.gsize) {   // headers (item 0: global body ids)
-            const int id = dst[q];
-            int b1, b2;
-            if (pass == 0) {
-                const float4 bod = prow(w, buf, PR_BODIES, id);
-                b1 = as_int(bod.z); b2 = as_int(bod.w);
-            } else {
-                const int4 ji = w.j_info[id];
-                b1 = ji.x; b2 = ji.y;
-            }
-            int id1 = body_is_sim(w, b1) ? b1 : NO_BODY;
-            int id2 = body_is_sim(w, b2) ? b2 : NO_BODY;
-            if (w.any_extra) (pass == 0 ? w.cons_key : w.j_key)[q] = w.b_key[id1 != NO_BODY ? b1 : b2];   // (both ends share the island)
-            if (pass == 0) {   // contact_with_twist_friction.rs:71-84
-                const int rel_dom = relative_dominance(w, b1, b2);
-                if (rel_dom > 0) id1 = NO_BODY;
-                if (rel_dom < 0) id2 = NO_BODY;
-                w.cons_hdr[q] = make_int4(id, id1, id2, 0);
-            } else {
-                w.j_sched_ids[q] = make_int4(id, id1, id2, 0);
-            }
-        }
+        for (int q = s0 + ctx.gtid; q < s1; q += ctx.gsize) write_sched_header(w, buf, t.joints, false, q, t.dst[q]);   // (global ids)
         ctx.grid_sync();
     }
     // S10 per-item counting sort by colour stage (one CTA per item), headers for the solver.
@@ -1459,21 +1481,13 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         RB_SHARED int hist[NUM_COLORS + 1];
         RB_SHARED int curs[NUM_COLORS + 1];
         for (int pass = 0; pass < 2; ++pass) {  // 0: contacts, 1: joints
-            const int* starts = pass == 0 ? w.item_cons_start : w.item_joint_start;
-            int s0 = starts[it], s1 = starts[it + 1];
+            const SchedSide t = sched_side(w, pass == 1);
+            int s0 = t.starts[it], s1 = t.starts[it + 1];
             if (pass == 0 && s1 > w.cons_cap) s1 = s0 > w.cons_cap ? s0 : w.cons_cap;
-            const int* src = pass == 0 ? w.cons_pair_tmp : w.joint_tmp;
-            int* dst = pass == 0 ? w.cons_pair : w.joint_sched;
-            int* offs = (pass == 0 ? w.item_color_off : w.item_jcolor_off) + (size_t)it * (NUM_COLORS + 1);
-            const int* cpos = pass == 0 ? w.color_pos : w.jcolor_pos;
+            int* offs = t.offs + (size_t)it * (NUM_COLORS + 1);
             for (int c = ctx.btid; c <= NUM_COLORS; c += ctx.bsize) { hist[c] = 0; curs[c] = 0; }
             ctx.block_sync();
-            for (int q = s0 + ctx.btid; q < s1; q += ctx.bsize) {
-                int id = src[q];
-                int color = pass == 0 ? as_int(prow(w, buf, PR_INFO, id).w) : w.j_info[id].w;
-                if (color > COLOR_OVERFLOW) color = COLOR_OVERFLOW;
-                atomic_add(&hist[cpos[color]], 1);
-            }
+            for (int q = s0 + ctx.btid; q < s1; q += ctx.bsize) atomic_add(&hist[t.stage(w, buf, t.src[q])], 1);
             ctx.block_sync();
             if (ctx.btid == 0) {
                 int run = 0;
@@ -1481,51 +1495,23 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
             }
             ctx.block_sync();
             for (int q = s0 + ctx.btid; q < s1; q += ctx.bsize) {
-                int id = src[q];
-                int color = pass == 0 ? as_int(prow(w, buf, PR_INFO, id).w) : w.j_info[id].w;
-                if (color > COLOR_OVERFLOW) color = COLOR_OVERFLOW;
-                int p = cpos[color];
+                int id = t.src[q];
+                int p = t.stage(w, buf, id);
                 int l = atomic_add(&curs[p], 1);
-                dst[s0 + hist[p] + l] = id;
+                t.dst[s0 + hist[p] + l] = id;
             }
             ctx.block_sync();
             // the overflow colour is solved sequentially: order it by index
-            if (ctx.btid == 0 && cpos[COLOR_OVERFLOW] >= 0) {
-                int p = cpos[COLOR_OVERFLOW];
-                int a = s0 + offs[p], e = s0 + offs[p + 1];
-                for (int x = a + 1; x < e; ++x) {
-                    int v = dst[x], y = x;
-                    while (y > a && dst[y - 1] > v) { dst[y] = dst[y - 1]; --y; }
-                    dst[y] = v;
-                }
+            if (ctx.btid == 0 && t.cpos[COLOR_OVERFLOW] >= 0) {
+                int p = t.cpos[COLOR_OVERFLOW];
+                insertion_sort(t.dst + s0 + offs[p], offs[p + 1] - offs[p]);
             }
             ctx.block_sync();
-            // headers
-            for (int q = s0 + ctx.btid; q < s1; q += ctx.bsize) {
-                int id = dst[q];
-                int b1, b2;
-                if (pass == 0) {
-                    float4 bod = prow(w, buf, PR_BODIES, id);
-                    b1 = as_int(bod.z); b2 = as_int(bod.w);
-                } else {
-                    int4 ji = w.j_info[id];
-                    b1 = ji.x; b2 = ji.y;
-                }
-                int id1 = body_is_sim(w, b1) ? (it == 0 ? b1 : w.body_local[b1]) : NO_BODY;
-                int id2 = body_is_sim(w, b2) ? (it == 0 ? b2 : w.body_local[b2]) : NO_BODY;
-                if (w.any_extra) (pass == 0 ? w.cons_key : w.j_key)[q] = w.b_key[id1 != NO_BODY ? b1 : b2];
-                if (pass == 0) {   // contact_with_twist_friction.rs:71-84
-                    const int rel_dom = relative_dominance(w, b1, b2);
-                    if (rel_dom > 0) id1 = NO_BODY;
-                    if (rel_dom < 0) id2 = NO_BODY;
-                }
-                if (pass == 0) w.cons_hdr[q] = make_int4(id, id1, id2, 0);
-                else w.j_sched_ids[q] = make_int4(id, id1, id2, 0);
-            }
+            for (int q = s0 + ctx.btid; q < s1; q += ctx.bsize) write_sched_header(w, buf, t.joints, true, q, t.dst[q]);   // (item-local ids)
             ctx.block_sync();
             // per-body adjacency of the contact constraints, in stage (= slot) order: entry = slot * 2 + side.
             // The body-centric warm start of the shared-memory items walks it (rb_solver.cuh).
-            if (pass == 0 && it > 0) {
+            if (pass == 0) {
                 const int lb0 = w.item_body_start[it], lb1 = w.item_body_start[it + 1];
                 for (int l = lb0 + ctx.btid; l < lb1; l += ctx.bsize) w.adj_cnt[l] = 0;
                 ctx.block_sync();
@@ -1546,15 +1532,8 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
                     if (h.z >= 0) w.adj_list[w.adj_off[lb0 + h.z] + atomic_add(&w.adj_cnt[lb0 + h.z], 1)] = (q - s0) * 2 + 1;
                 }
                 ctx.block_sync();
-                for (int l = lb0 + ctx.btid; l < lb1; l += ctx.bsize) {   // order every short list by slot
-                    int* a = w.adj_list + w.adj_off[l];
-                    const int n = w.adj_cnt[l];
-                    for (int x = 1; x < n; ++x) {
-                        int v = a[x], y = x;
-                        while (y > 0 && a[y - 1] > v) { a[y] = a[y - 1]; --y; }
-                        a[y] = v;
-                    }
-                }
+                for (int l = lb0 + ctx.btid; l < lb1; l += ctx.bsize)   // order every short list by slot
+                    insertion_sort(w.adj_list + w.adj_off[l], w.adj_cnt[l]);
                 ctx.block_sync();
             }
         }
@@ -1569,21 +1548,14 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         for (int c = ctx.gtid; c <= ORDER_BUCKETS; c += ctx.gsize) { hist[c] = 0; if (c < ORDER_BUCKETS) curs[c] = 0; }
         ctx.grid_sync();
         for (int it = 1 + ctx.gtid; it < nitems; it += ctx.gsize) {
-            int nbod = w.item_body_start[it + 1] - w.item_body_start[it];
-            int work = (w.item_cons_start[it + 1] - w.item_cons_start[it]) + (w.item_joint_start[it + 1] - w.item_joint_start[it]);
-            if (nbod == 0 && work == 0) continue;
-            int cost = nbod > work ? nbod : work;
-            atomic_add(&hist[ORDER_BUCKETS - 1 - (cost < ORDER_BUCKETS ? cost : ORDER_BUCKETS - 1)], 1);
+            const int k = item_order_bucket(w, it);
+            if (k >= 0) atomic_add(&hist[k], 1);
         }
         ctx.grid_sync();
         grid_exclusive_scan(ctx, hist, hist, ORDER_BUCKETS + 1, w.scan_tmp);
         for (int it = 1 + ctx.gtid; it < nitems; it += ctx.gsize) {
-            int nbod = w.item_body_start[it + 1] - w.item_body_start[it];
-            int work = (w.item_cons_start[it + 1] - w.item_cons_start[it]) + (w.item_joint_start[it + 1] - w.item_joint_start[it]);
-            if (nbod == 0 && work == 0) continue;
-            int cost = nbod > work ? nbod : work;
-            int k = ORDER_BUCKETS - 1 - (cost < ORDER_BUCKETS ? cost : ORDER_BUCKETS - 1);
-            w.item_order[hist[k] + atomic_add(&curs[k], 1)] = it;
+            const int k = item_order_bucket(w, it);
+            if (k >= 0) w.item_order[hist[k] + atomic_add(&curs[k], 1)] = it;
         }
         ctx.grid_sync();
     }
@@ -1594,8 +1566,6 @@ RB_PHASE void section_schedule(const Ctx& ctx, const World& w) {
         st->nlarge_bodies = w.item_body_start[1] - w.item_body_start[0];
         st->nlarge_cons = w.item_cons_start[1] - w.item_cons_start[0];
         st->nlarge_joints = w.item_joint_start[1] - w.item_joint_start[0];
-        int nisl = 0;
-        (void)nisl;
         st->sched_dirty = 0;
         st->sched_ran = 1;
     }

@@ -1170,11 +1170,12 @@ RB_PHASE void phase_force_events(const Ctx& ctx, const World& w) {
     const int buf = st->cur, np = st->npairs;
     for (int i = ctx.gtid; i < np; i += ctx.gsize) {
         float4 info = prow(w, buf, PR_INFO, i);
+        if (!pair_has_forces(w, info)) continue;
         const int nsc = as_int(info.z);
-        if (nsc <= 0 || (w.has_filters && (as_int(info.x) & 32))) continue;   // (a pair without forces raises no force event)
         const unsigned long long key = w.pb[buf].key[i];
         const int c1 = (int)(key >> 32), c2 = (int)(key & 0xffffffffu);
-        const float t1 = (w.c_events[c1] & 2) ? w.c_force_thr[c1] : FMAX32, t2 = (w.c_events[c2] & 2) ? w.c_force_thr[c2] : FMAX32;
+        const float t1 = (w.c_events[c1] & EV_CONTACT_FORCE) ? w.c_force_thr[c1] : FMAX32;
+        const float t2 = (w.c_events[c2] & EV_CONTACT_FORCE) ? w.c_force_thr[c2] : FMAX32;
         const float threshold = min2(t1, t2);
         if (!(threshold < FMAX32)) continue;
         const float4 bod = prow(w, buf, PR_BODIES, i);
@@ -1193,12 +1194,12 @@ RB_PHASE void phase_force_events(const Ctx& ctx, const World& w) {
             const vec3 tf = (n * total) * w.prm.inv_dt_full;
             const int slot = atomic_add(&st->nev_force, 1);
             if (slot < w.ev_cap) {
-                w.ev_force[slot] = make_float4(as_float_i(c1), as_float_i(c2), as_float_i((flags & 8) ? 0 : 1), as_float_i(w.step_index));
+                w.ev_force[slot] = make_float4(as_float_i(c1), as_float_i(c2), as_float_i((flags & PF_FORCE_EVENT) ? 0 : 1), as_float_i(w.step_index));
                 w.ev_force[w.ev_cap + slot] = f4(tf, magnitude);
                 w.ev_force[2 * w.ev_cap + slot] = f4(maxi > 0.0f ? n : zero3(), maxi * w.prm.inv_dt_full);
-            } else RB_RAISE(w, -4);
-            flags |= 8;
-        } else flags &= ~8;
+            } else RB_RAISE(w, STATUS_CAPACITY);
+            flags |= PF_FORCE_EVENT;
+        } else flags &= ~PF_FORCE_EVENT;
         if (flags != as_int(info.x)) { info.x = as_float_i(flags); prow(w, buf, PR_INFO, i) = info; }
     }
 }
@@ -1303,7 +1304,7 @@ RB_HD void body_writeback(const World& w, const B& bd, int b, int id) {
         const int slot = atomic_add(&w.st->nquarantine, 1);
         if (slot < w.nb) w.quarantine[slot] = b;
         w.st->lists_dirty = 3; w.st->bp_dirty = 1; w.st->sched_dirty = 1;
-        RB_RAISE(w, -5);
+        RB_RAISE(w, STATUS_NONFINITE);
         return;
     }
     if (P.ccd && w.b_type[b] == BODY_DYNAMIC && ccd_is_moving_fast(P, xyz(w.b_lcom_im[b]), ccd_op, np, ccd_ext, ccd_thick)) {

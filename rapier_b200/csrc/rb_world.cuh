@@ -44,9 +44,7 @@ struct HullTables {
 
 // ---- persistent pair record rows (float4 each) ----
 enum PairRow {
-    PR_INFO = 0,   // int bits: x flags(bit0 has_recycle, bit1 pending colour, bit2 colouring scratch, bit3 force event emitted last step, bit4 sensor pair intersecting,
-                   //   worlds with collider filters only: bit5 contacts without forces (solver groups fail or no dynamic body),
-                   //   bit6 the narrow phase has updated the pair at least once), y npts, z nsc, w colour
+    PR_INFO = 0,   // int bits: x flags (PF_*), y npts, z nsc, w colour
     PR_BODIES,     // int bits: x colour_body0, y colour_body1, z body1, w body2 (-1 none)
     PR_RT,         // recycle pos12.t xyz, w max_extent
     PR_RQ,         // recycle pos12.q
@@ -65,6 +63,24 @@ enum PairRow {
     PR_A2 = PR_A1 + MAX_PTS,    // [4] anchor2 xyz
     PR_ROWS = PR_A2 + MAX_PTS
 };
+
+// PR_INFO.x flag bits
+constexpr int PF_RECYCLE = 1;         // PR_RT .. PR_ROT2 hold a valid recycling base (contact recycling)
+constexpr int PF_PENDING_COLOR = 2;   // began touching: awaits a colour from the deferred greedy pass
+constexpr int PF_COLORED = 4;         // coloured in the current round of that pass (scratch, cleared by the round)
+constexpr int PF_FORCE_EVENT = 8;     // a contact-force event was emitted for the pair last step
+constexpr int PF_SENSOR_HIT = 16;     // sensor pair: the shapes intersect
+// worlds with collider filters only:
+constexpr int PF_FORCELESS = 32;      // contacts without forces (solver groups fail or no dynamic body)
+constexpr int PF_UPDATED = 64;        // the narrow phase has updated the pair at least once
+
+// World::c_events bits: ActiveEvents (the same values as RB_EVENT_*) and whether the collider is a sensor
+constexpr int EV_COLLISION = 1, EV_CONTACT_FORCE = 2, EV_SENSOR = 4;
+
+// Statuses raised on the device (RB_RAISE); the same values as RB_ERR_CAPACITY, RB_ERR_NONFINITE and RB_ERR_SHARD
+constexpr int STATUS_CAPACITY = -4;   // a device-side table overflowed
+constexpr int STATUS_NONFINITE = -5;  // a body state went non-finite (quarantined)
+constexpr int STATUS_SHARD = -6;      // a contact formed with a dynamic body simulated by another rank
 
 // ---- per-step constraint record rows (float4 each), index = slot in the schedule ----
 enum ConsRow {
@@ -196,7 +212,7 @@ struct World {
     float4* c_mat;                    // friction, restitution, contact_skin
     int2* c_rules;
     uint2* c_groups;
-    int* c_events;                    // ActiveEvents bits (1 = collision events, 2 = contact force events) | 4 = the collider is a sensor
+    int* c_events;                    // EV_* bits
     int has_sensors;                  // some collider is a sensor (Collider::is_sensor): intersection-only pairs exist
     int has_filters;                  // some collider holds filters other than the defaults (c_filter); no other world reads c_filter
     float* c_force_thr;               // contact_force_event_threshold
